@@ -222,19 +222,10 @@ int cmx_create(cmx_ctx **out, int device, const cmx_params *params) {
     CUC(cudaMalloc(&L.ctr, sizeof(Counters)));
     CUC(cudaMalloc(&L.d_count, sizeof(int) * 4));
   }
-  // MAPQ tables from the host libm, so truncations match the reference bit for bit (mapping_generator.h:920-1022)
   {
     std::vector<double> il(65536, 0.0);
-    const int coef_frac = log(50);
-    for (int a = 2; a < 65536; ++a) il[a] = coef_frac / log((unsigned short)a);
     std::vector<int> thr(96, 0x7fffffff);
-    for (int v = 0; v < 96; ++v) {  // smallest n >= 0 with (int)(4.343*log(n+1)+0.499) >= v (monotone in n)
-      long long lo = 0, hi = 0x7ffffffeLL;
-      auto pen = [](long long n) { return (int)(4.343 * log((double)(n + 1)) + 0.499); };
-      if (pen(hi) < v) { thr[v] = 0x7fffffff; continue; }
-      while (lo < hi) { const long long mid = (lo + hi) / 2; if (pen(mid) >= v) hi = mid; else lo = mid + 1; }
-      thr[v] = (int)lo;
-    }
+    mapq_tables_fill(il.data(), thr.data());
     CUC(cudaMalloc(&ctx->inv_log, 65536 * sizeof(double)));
     CUC(cudaMalloc(&ctx->pen_thr, 96 * sizeof(int)));
     CUC(cudaMemcpy(ctx->inv_log, il.data(), 65536 * sizeof(double), cudaMemcpyHostToDevice));
@@ -576,43 +567,22 @@ int cmx_download_index(cmx_ctx *ctx, uint32_t *n_buckets, uint32_t *n_keys, uint
 }
 
 // ---------------------------------------------------------------------------------------------------
-static size_t tier_bytes(const Caps &c, size_t slots, bool interleaved, size_t *o) {  // o[11]
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t r = off; off = (off + bytes + 255) / 256 * 256; return r; };
-  const size_t R = 2 * slots;
-  const size_t Rm = interleaved ? 2 * ((slots + 31) / 32 * 32) : R;  // minimizer records: whole groups of 32 pairs
-  o[0] = take(R * sizeof(ReadMeta));
-  o[1] = take(slots * sizeof(PairMeta));
-  o[2] = take(interleaved ? 0 : R * c.maxmm * 8);  // hashes: tier 0 never stores them
-  o[3] = take(Rm * c.maxmm * 8);
-  o[4] = take(Rm * c.maxmm * 4);
-  o[5] = take(R * 2 * (size_t)c.hc * 8);
-  o[6] = take(R * 6 * (size_t)c.cc * 8);
-  o[7] = take(R * 6 * (size_t)c.cc);
-  o[8] = take(R * 2 * (size_t)c.mc * 8);
-  o[9] = take(R * 2 * (size_t)c.mc * 2);
-  o[10] = take(R * 2 * (size_t)c.mc * 4);
-  return off;
-}
 static cudaError_t tier_prepare(Tier &t, int n_slots, const int *pair_list, bool interleaved) {
+  size_t o[SCRATCH_ARRAYS];
   if (n_slots > t.slots_cap) {
-    size_t o[11];
     const size_t want_slots = (size_t)n_slots + n_slots / 8 + 16;
-    const size_t bytes = tier_bytes(t.caps, want_slots, interleaved, o);
+    const size_t bytes = scratch_layout(t.caps, want_slots, interleaved, o);
     release(t.mem);
     cudaError_t e = ensure(t.mem, bytes);
     if (e != cudaSuccess) return e;
     t.slots_cap = (int)want_slots;
   }
-  size_t o[11];
-  tier_bytes(t.caps, t.slots_cap, interleaved, o);
-  char *b = (char *)t.mem.p;
+  scratch_layout(t.caps, t.slots_cap, interleaved, o);
+  char *a[SCRATCH_ARRAYS];
+  for (int i = 0; i < SCRATCH_ARRAYS; ++i) a[i] = (char *)t.mem.p + o[i];
   Scratch &S = t.view;
   S.caps = t.caps; S.n_slots = n_slots; S.pair_list = pair_list; S.mm_il = interleaved ? 1 : 0;
-  S.rmeta = (ReadMeta *)(b + o[0]); S.pmeta = (PairMeta *)(b + o[1]);
-  S.mm_hash = (u64 *)(b + o[2]); S.mm_val = (u64 *)(b + o[3]); S.mm_pos = (u32 *)(b + o[4]);
-  S.hits = (u64 *)(b + o[5]); S.cand_pos = (u64 *)(b + o[6]); S.cand_cnt = (u8 *)(b + o[7]);
-  S.map_pos = (u64 *)(b + o[8]); S.map_err = (short *)(b + o[9]); S.map_split = (int *)(b + o[10]);
+  scratch_bind(S, a);
   t.n_slots = n_slots; t.pair_list = pair_list;
   return cudaSuccess;
 }

@@ -94,6 +94,33 @@ struct Scratch {
   int *map_split;        // [2n][2][mc]   split_sites word (draft_mapping_generator.cc:550-554)
 };
 
+// Layout of one tier's scratch for `slots` pair slots, its arrays in the order of Scratch's pointers (rmeta .. map_split):
+// size[i] = bytes of array i, off[i] = its offset in one allocation where every array starts on a 256-byte boundary.
+// Returns the size of that allocation.
+#define SCRATCH_ARRAYS 11
+inline size_t scratch_layout(const Caps &c, size_t slots, bool interleaved, size_t *off, size_t *size = nullptr) {
+  const size_t R = 2 * slots;
+  const size_t Rm = interleaved ? 2 * ((slots + 31) / 32 * 32) : R;  // minimizer records: whole groups of 32 pairs
+  const size_t sz[SCRATCH_ARRAYS] = {R * sizeof(ReadMeta), slots * sizeof(PairMeta),
+                                     interleaved ? 0 : R * c.maxmm * 8,  // hashes: tier 0 never stores them
+                                     Rm * c.maxmm * 8, Rm * c.maxmm * 4, R * 2 * (size_t)c.hc * 8, R * 6 * (size_t)c.cc * 8, R * 6 * (size_t)c.cc,
+                                     R * 2 * (size_t)c.mc * 8, R * 2 * (size_t)c.mc * 2, R * 2 * (size_t)c.mc * 4};
+  size_t end = 0;
+  for (int i = 0; i < SCRATCH_ARRAYS; ++i) {
+    off[i] = end;
+    if (size) size[i] = sz[i];
+    end = (end + sz[i] + 255) / 256 * 256;
+  }
+  return end;
+}
+// Points S's arrays at a[0 .. SCRATCH_ARRAYS), in scratch_layout's order.
+inline void scratch_bind(Scratch &S, char *const *a) {
+  S.rmeta = (ReadMeta *)a[0]; S.pmeta = (PairMeta *)a[1];
+  S.mm_hash = (u64 *)a[2]; S.mm_val = (u64 *)a[3]; S.mm_pos = (u32 *)a[4];
+  S.hits = (u64 *)a[5]; S.cand_pos = (u64 *)a[6]; S.cand_cnt = (u8 *)a[7];
+  S.map_pos = (u64 *)a[8]; S.map_err = (short *)a[9]; S.map_split = (int *)a[10];
+}
+
 __device__ __forceinline__ int slot_pair(const Scratch &S, int slot) { return S.pair_list ? S.pair_list[slot] : slot; }
 
 // utils.h:87-104: A/a=0 C/c=1 G/g=2 T/t=3, everything else 4.  Branch-free on purpose: a chain of ternaries

@@ -176,6 +176,7 @@ __global__ void fold_runs_kernel(const u64 *hash, const u64 *hit, const u32 *mul
     cudaError_t e_ = (call);                                                                 \
     if (e_ != cudaSuccess) { *err = std::string(#call) + ": " + cudaGetErrorString(e_); goto fail_; } \
   } while (0)
+#ifndef CMX_HOST_EMU  // (CUDA host code: the host emulation of a CTA runs the kernels above in this sequence itself)
 
 static int build_index_on_device(const u8 *d_ref, const std::vector<u64> &off, const std::vector<u32> &len, int k, int w,
                                  IndexBuildResult *res, std::string *err) {
@@ -254,3 +255,4 @@ fail_:
   cudaFree(d_cnt); cudaFree(d_tmp); cudaFree(d_multi); cudaFree(d_occidx); cudaFree(d_occ); cudaFree(d_slots);
   return -2;
 }
+#endif

@@ -10,6 +10,19 @@ struct MapqTables {
   const double *inv_log;  // [65536]: 3 / log(alignment_length) as computed by the host libm (mapping_generator.h:956-958)
   const int *pen_thr;     // [96]: smallest n with (int)(4.343*log(n+1)+0.499) >= v   (mapping_generator.h:964-967)
 };
+// The two tables from the host libm, so truncations match the reference bit for bit (mapping_generator.h:920-1022).
+inline void mapq_tables_fill(double *inv_log, int *pen_thr) {
+  const int coef_frac = log(50);
+  inv_log[0] = inv_log[1] = 0.0;
+  for (int a = 2; a < 65536; ++a) inv_log[a] = coef_frac / log((unsigned short)a);
+  for (int v = 0; v < 96; ++v) {  // smallest n >= 0 with (int)(4.343*log(n+1)+0.499) >= v (monotone in n)
+    long long lo = 0, hi = 0x7ffffffeLL;
+    auto pen = [](long long n) { return (int)(4.343 * log((double)(n + 1)) + 0.499); };
+    if (pen(hi) < v) { pen_thr[v] = 0x7fffffff; continue; }
+    while (lo < hi) { const long long mid = (lo + hi) / 2; if (pen(mid) >= v) hi = mid; else lo = mid + 1; }
+    pen_thr[v] = (int)lo;
+  }
+}
 
 struct Counters {  // device-side statistics (atomics)
   u64 n_minimizers, n_probe_steps, n_found, n_occ_reads, n_verified, n_candidates, n_mapped, n_unique, n_overflow;
@@ -32,6 +45,7 @@ __device__ __forceinline__ u8 code_char(u32 c) { return c == 0 ? 'A' : c == 1 ? 
 
 // Counter updates: every lane adds to the same address, and same-address atomics serialise in L2 at about one
 // per clock, so the lanes that are here together add up first and one of them issues the atomic.
+#ifndef CMX_HOST_EMU  // (__activemask has no host equivalent: the host emulation of a CTA supplies plain atomics)
 __device__ __forceinline__ void agg_add(u64 *addr, u64 v) {
   const unsigned m = __activemask();
   const unsigned s_ = __reduce_add_sync(m, (unsigned)v);
@@ -46,6 +60,7 @@ __device__ __forceinline__ int agg_append(int *count) {
   base = __shfl_sync(m, base, leader);
   return base + __popc(m & ((1u << lane) - 1u));
 }
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // K0: per pair — length filter (chromap.h:911-916) and adapter trimming (chromap.cc:176-289).

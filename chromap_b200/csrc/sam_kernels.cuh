@@ -95,7 +95,7 @@ SAM_HD int sam_band_align(int rlen, int e, int match, int mismatch, int o_del, i
   return n;
 }
 
-#ifdef __CUDACC__
+#if defined(__CUDACC__) || defined(CMX_HOST_EMU)
 struct OutSam {  // == cmx_sam_record
   u32 read_id, rid;
   u32 pos[2], end[2];  // 0-based inclusive reference span of mate 1 / mate 2 (single-end: index 0)

@@ -13,6 +13,7 @@
 #include "pipeline_kernels.cuh"
 
 // ---- mbarrier + bulk copy (PTX ISA 8.x, sm_90+) ---------------------------------------------------------------------
+#ifndef CMX_HOST_EMU  // (the host emulation of a CTA supplies an mbarrier word and a copy that signals its bytes)
 __device__ __forceinline__ u32 smem_u32(const void *p) { return (u32)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(u64 *bar, u32 count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -36,6 +37,7 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, u32 bytes, 
                "r"(smem_u32(bar))
                : "memory");
 }
+#endif
 
 // ---- the kernel ------------------------------------------------------------------------------------------------------
 #define SF_TILE 64   // pairs per tile

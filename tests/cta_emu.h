@@ -3,24 +3,41 @@
 // One OS thread per CUDA thread; barriers are counting barriers that threads may leave; a warp shuffle is an exchange through a per-warp buffer
 // bracketed by two warp barriers.  Every lane of a warp must reach a shuffle (true of the functions under test: their scans
 // are unconditional).  Not a performance tool.
+// The kernel headers test CMX_HOST_EMU to leave out the few spots that have no host form (the end of this file supplies them).
 #pragma once
 #include <pthread.h>
+#include <sched.h>
 
 #include <atomic>
 #include <mutex>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
 #include <functional>
+#include <numeric>
+#include <random>
+#include <string>
 #include <thread>
 #include <vector>
+
+#define CMX_HOST_EMU 1
 
 typedef unsigned long long u64;
 typedef unsigned int u32;
 typedef unsigned char u8;
 #define __device__
+#define __host__
 #define __forceinline__ inline
+#define __noinline__
 #define __global__
+#define __shared__ static
+#define __launch_bounds__(...)
+#define __ldg(p) (*(p))
+struct ulonglong2 { u64 x, y; };
 using std::max;
 using std::min;
 
@@ -171,4 +188,56 @@ static inline void emu_grid_serial(int grid, int nt, const std::function<void()>
       threadIdx.x = t; blockDim.x = nt; blockIdx.x = b; gridDim.x = grid;
       body();
     }
+}
+
+// ---- dynamic shared memory: tests/emu.py rewrites `extern __shared__ T name[];` as `T *name = (T *)g_dyn_smem;`, the test
+// points it at a buffer of the launch's size
+static u64 *g_dyn_smem = nullptr;
+
+// ---- atomics and intrinsics
+static inline u64 atomicAdd(u64 *p, u64 v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+static inline int atomicAdd(int *p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+static inline u32 atomicAdd(u32 *p, u32 v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+static inline int atomicExch(int *p, int v) { return __atomic_exchange_n(p, v, __ATOMIC_RELAXED); }
+static inline u64 atomicCAS(u64 *p, u64 cmp, u64 val) { __atomic_compare_exchange_n(p, &cmp, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED); return cmp; }
+template <typename T> static inline T emu_atomic_max(T *p, T v) { T o = __atomic_load_n(p, __ATOMIC_RELAXED); while (o < v && !__atomic_compare_exchange_n(p, &o, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return o; }
+template <typename T> static inline T emu_atomic_min(T *p, T v) { T o = __atomic_load_n(p, __ATOMIC_RELAXED); while (v < o && !__atomic_compare_exchange_n(p, &o, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return o; }
+static inline u64 atomicMax(u64 *p, u64 v) { return emu_atomic_max(p, v); }
+static inline u32 atomicMax(u32 *p, u32 v) { return emu_atomic_max(p, v); }
+static inline u32 atomicMin(u32 *p, u32 v) { return emu_atomic_min(p, v); }
+// pipeline_kernels.cuh's counter helpers: on the device one atomic per group of converged lanes, here one per thread
+static inline void agg_add(u64 *addr, u64 v) { atomicAdd(addr, v); }
+static inline int agg_append(int *count) { return atomicAdd(count, 1); }
+static inline double __dmul_rn(double a, double b) { return a * b; }   // (built with -ffp-contract=off: no FMA contraction either)
+static inline double __dadd_rn(double a, double b) { return a + b; }
+static inline double __ddiv_rn(double a, double b) { return a / b; }
+static inline double __dsqrt_rn(double a) { return std::sqrt(a); }
+static inline u32 __funnelshift_r(u32 lo, u32 hi, u32 s) { return (u32)((((u64)hi << 32) | lo) >> (s & 31)); }
+
+// ---- host equivalents of seed_front.cuh's six PTX wrappers (mbarrier + cp.async.bulk).
+// An mbarrier word: bits 0-31 = bytes still expected, bits 32-47 = arrivals still expected, bits 48-63 = completed phases.  The
+// "copy engine" copies at issue time and then signals its bytes, like complete_tx.
+static inline void emu_mbar_settle(u64 *bar) {   // a phase completes when no arrival and no byte is outstanding: re-arm with one arrival
+  u64 v = __atomic_load_n(bar, __ATOMIC_ACQUIRE);
+  if ((v & 0xFFFFFFFFFFFFull) == 0) __atomic_store_n(bar, ((v >> 48) + 1) << 48 | (1ull << 32), __ATOMIC_RELEASE);
+}
+static inline u32 smem_u32(const void *p) { return (u32)(size_t)p; }
+static inline void mbar_init(u64 *bar, u32 count) { __atomic_store_n(bar, (u64)count << 32, __ATOMIC_RELEASE); }
+static inline void mbar_fence_init() {}
+static inline void mbar_arrive_expect_tx(u64 *bar, u32 bytes) {   // (called by one thread, before its copies)
+  u64 v = __atomic_load_n(bar, __ATOMIC_ACQUIRE);
+  v = (v & 0xFFFF000000000000ull) | ((((v >> 32) & 0xFFFF) - 1) << 32) | (u64)((u32)v + bytes);
+  __atomic_store_n(bar, v, __ATOMIC_RELEASE);
+  emu_mbar_settle(bar);
+}
+static inline bool mbar_try_wait(u64 *bar, u32 parity) {
+  const bool done = (((__atomic_load_n(bar, __ATOMIC_ACQUIRE) >> 48) & 1u) != parity);
+  if (!done) sched_yield();
+  return done;
+}
+static inline void bulk_g2s(void *dst, const void *src, u32 bytes, u64 *bar) {
+  memcpy(dst, src, bytes);
+  u64 v = __atomic_load_n(bar, __ATOMIC_ACQUIRE);
+  __atomic_store_n(bar, (v & 0xFFFFFFFF00000000ull) | (u64)((u32)v - bytes), __ATOMIC_RELEASE);
+  emu_mbar_settle(bar);
 }

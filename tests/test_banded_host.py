@@ -4,27 +4,12 @@ folded into one `banded_align_dropoff`) compiled for the HOST and compared with 
 (pinned to the reference binary by tests/test_oracle_golden.py) on random windows: substitutions, indels, N's, soft-masked
 reference bases, chimeric reads, every e the path accepts.  The same comparison runs on the GPU in the stage tests; this one
 keeps the device formulation honest on machines without one."""
-import os
-import subprocess
+from tests import emu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <string>
-#include <vector>
-typedef unsigned long long u64; typedef unsigned int u32; typedef unsigned char u8;
-#define __device__
-#define __forceinline__ inline
-static inline u32 base_code(u8 c) { switch (c) { case 'A': case 'a': return 0; case 'C': case 'c': return 1; case 'G': case 'g': return 2; case 'T': case 't': return 3; default: return 4; } }
+MAIN = r'''
 extern "C" int orc_banded_align(int e, const char *pattern, const char *text, int read_len, int *end_pos);
 extern "C" void orc_banded_traceback(int e, int min_errors, const char *pattern, const char *text, int read_len, int *start_pos);
 extern "C" int orc_align_dropoff(int e, const char *pattern, const char *text, int read_len, int from_3_end, int *end_pos, int *read_len_out);
-'''
-
-POST = r'''
 static std::string mutate(const std::string &ref, int off, int L, int n_edit, bool chimera) {
   std::string read;
   int p = off;
@@ -96,23 +81,8 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_device_banded_aligners_equal_the_oracle(tmp_path):
-    k = open(os.path.join(ROOT, "chromap_b200", "csrc", "pipeline_kernels.cuh")).read()
-    body = _between(k, "struct PatPlanes", "__device__ __forceinline__ bool valid_cand")
-    body += _between(k, "template <typename PatC, typename TxtC>\n__device__ __forceinline__ int banded_traceback_dp", "// IEEE double ops without FMA contraction")
-    body += _between(k, "template <typename PatF, typename TxtF>\n__device__ __forceinline__ int banded_align_dropoff", "struct SplitResult")
-    src = tmp_path / "t.cc"
-    src.write_text(PRE + body + POST)
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=900)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN, timeout=900)
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-1200:]
     # the interesting branches were really taken
     f = dict(kv.split("=") for kv in out.stdout.replace("(bit-vector path ", "dp=").replace(")", "").split() if "=" in kv)

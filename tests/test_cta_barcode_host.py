@@ -3,38 +3,7 @@ CorrectBarcodeAt, chromap.cc:572-799, for --bc-error-threshold 0 and 1) run UNCH
 against the oracle's `correct_barcode` (pinned to the reference binary by the scATAC golden files): whitelist membership, one
 substitution, one N, ties broken by (score, index, base), the posterior threshold, qualities clamped to [3, 40], abundances from
 a sampled count table; keys and accept flags of every barcode and both counters."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-#include <cmath>
-#include <cstring>
-#include <cstdio>
-#include <cstdlib>
-#include <random>
-#include <string>
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __launch_bounds__(...)
-#define __ldg(p) (*(p))
-static u64 *g_dyn_smem = nullptr;
-static inline u64 atomicAdd(u64 *p, u64 v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline int atomicAdd(int *p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline int atomicExch(int *p, int v) { return __atomic_exchange_n(p, v, __ATOMIC_RELAXED); }
-static inline u64 atomicCAS(u64 *p, u64 cmp, u64 val) { __atomic_compare_exchange_n(p, &cmp, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED); return cmp; }
-static inline void agg_add(u64 *addr, u64 v) { atomicAdd(addr, v); }
-static inline int agg_append(int *count) { return atomicAdd(count, 1); }
-static inline double __dmul_rn(double a, double b) { return a * b; }
-static inline double __dadd_rn(double a, double b) { return a + b; }
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __dsqrt_rn(double a) { return std::sqrt(a); }
-static inline u32 __funnelshift_r(u32 lo, u32 hi, u32 s) { return (u32)((((u64)hi << 32) | lo) >> (s & 31)); }
-'''
+from tests import emu
 
 MAIN = r'''
 extern "C" {
@@ -111,24 +80,7 @@ int main(int argc, char **argv) {
 
 
 def test_barcode_correction_kernel_equals_the_oracle(tmp_path):
-    src_dir = os.path.join(ROOT, "chromap_b200", "csrc")
-    files = ["device_common.cuh", "minimizers.cuh", "pipeline_kernels.cuh"]
-    text = "\n".join(open(os.path.join(src_dir, f)).read() for f in files)
-    text = re.sub(r'#include [<"][^\n]*', "", text).replace("#pragma once", "")
-    text = re.sub(r'asm volatile\(.*?\)\s*;', ';', text)
-    text = re.sub(r"#pragma unroll[^\n]*", "", text)
-    text = re.sub(r"extern __shared__ (\w+) (\w+)\[\];", r"\1 *\2 = (\1 *)g_dyn_smem;", text)
-    a = text.index("// Counter updates: every lane adds to the same address")
-    b = text.index("// ------------------------------------------------------------------------------------------------\n// K0: per pair")
-    text = text[:a] + text[b:]
-    main = MAIN % dict(orc_h=os.path.join(ROOT, "oracle", "oracle_chromap.h"))
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + text + main.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-ffp-contract=off", "-std=c++20", "-pthread", "-w", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe), str(tmp_path)], capture_output=True, text=True, timeout=1200)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN % dict(orc_h=emu.ORACLE_H), args=[str(tmp_path)], timeout=1200)
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2500:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["in_whitelist"]) > 5000 and int(f["corrected"]) > 1000 and int(f["rejected"]) > 2000, out.stdout

@@ -1,37 +1,13 @@
 """Record emission of the CUDA path on the host emulation of a CTA (tests/cta_emu.h), kernels run UNCHANGED:
 `pairing_kernel` -> `emit_kernel` (warp-phased: chosen best pairs, the Hamming shortcut of BandedTraceback by the whole warp,
 the indel cases deferred to a list) + `emit_dp_kernel`, and `pairing_cta_kernel` -> `emit_cta_kernel` (best pairs counted per
-share, located by prefix sums), with the MAPQ tables built by the library's own table code (cut out of api.cu), against the
+share, located by prefix sums), with the MAPQ tables built by the library's own `mapq_tables_fill`, against the
 oracle's post-verification stage (`orc_emit_test` = the tail of its mapper: mapping_generator.h:160-253, :486-1192,
 mapping_generator.cc:110-143; pinned to the reference binary by tests/test_oracle_golden.py).  Draft mappings are real
 alignments of mutated reads (substitutions, indels, soft-masked reference bases) at planted copies, so the spans, the alignment
 lengths and with them every MAPQ branch (repetitive-seed scaling, second-best penalty, uint8 wrap, mate mixing, forced 0)
 are exercised; -n 1 .. 3 with the reservoir selection computed by libstdc++ exactly as the reference does."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-#include <cmath>
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __launch_bounds__(...)
-#define __ldg(p) (*(p))
-#define CTA_NT 128
-static u64 *g_dyn_smem = nullptr;
-static inline void atomicAdd(u64 *p, u64 v) { __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline int atomicAdd(int *p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline void agg_add(u64 *addr, u64 v) { atomicAdd(addr, v); }
-static inline int agg_append(int *count) { return atomicAdd(count, 1); }   // (the device version takes one atomic per group of converged lanes)
-static inline double __dmul_rn(double a, double b) { return a * b; }
-static inline double __dadd_rn(double a, double b) { return a + b; }
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __dsqrt_rn(double a) { return std::sqrt(a); }
-'''
+from tests import emu
 
 MAIN = r'''
 #include <cstdio>
@@ -49,11 +25,8 @@ static char comp(char c) { switch (c) { case 'A': case 'a': return 'T'; case 'C'
 static std::string revc(const std::string &s) { std::string r(s.rbegin(), s.rend()); for (auto &c : r) c = comp(c); return r; }
 int main() {
   std::mt19937 g(71);
-  std::vector<double> il_; std::vector<int> thr_;
-  {
-%(tables)s
-    il_ = il; thr_ = thr;
-  }
+  std::vector<double> il_(65536); std::vector<int> thr_(96);
+  mapq_tables_fill(il_.data(), thr_.data());
   MapqTables T{il_.data(), thr_.data()};
   long bad = 0, n_pairs = 0, n_records = 0, n_deferred = 0, multi = 0, mapq_hist[4] = {0, 0, 0, 0};
   for (int it = 0; it < 220; ++it) {
@@ -195,37 +168,8 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_emit_kernels_equal_the_oracles_post_verification_stage(tmp_path):
-    d = open(os.path.join(ROOT, "chromap_b200", "csrc", "device_common.cuh")).read()
-    k = open(os.path.join(ROOT, "chromap_b200", "csrc", "pipeline_kernels.cuh")).read()
-    c = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_pair_candidates.cuh")).read()
-    v = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_verify_pairing.cuh")).read()
-    api = open(os.path.join(ROOT, "chromap_b200", "csrc", "api.cu")).read()
-    tables = _between(api, "    std::vector<double> il(65536, 0.0);", "    CUC(cudaMalloc(&ctx->inv_log")
-    d = re.sub(r'asm volatile\(.*?\)\s*;', ';', d.replace("#include <cuda_runtime.h>", ""))
-    parts = [d,
-             _between(k, "struct MapqTables", "// Counter updates: every lane adds to the same address"),
-             _between(k, "struct PatPlanes", "// K3: per read — GenerateDraftMappings"),
-             _between(k, "template <typename Visit>\n__device__ __forceinline__ void pair_sweep(", "// ------------------------------------------------------------------------------------------------\n// K5: multi-mapper sampling"),
-             _between(k, "template <typename PatC, typename TxtC>\n__device__ __forceinline__ int banded_traceback_dp", "// compaction of per-pair records into read order"),
-             _between(k, "// same for (key, tag) pairs under `less`", "// candidate_processor.cc:283-342 with the sorted hits streamed"),
-             _between(c, "// ---- CTA-wide scans (one value per thread)", "// ---- MergeCandidates (candidate_processor.cc:345-414)"),
-             _between(v, "// Tally (min, #min, second distinct min, #second) of a multiset", "// GenerateDraftMappings for one read (non-split)."),
-             v[v.index("// Best-pair statistics for one pair by one CTA"):]]
-    body = re.sub(r"#pragma unroll[^\n]*", "", "\n".join(parts)).replace("#pragma once", "")
-    body = body.replace("extern __shared__ u64 smk[];", "u64 *smk = g_dyn_smem;")
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + body + (MAIN % dict(tables=tables.replace("%", "%%"))).replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-ffp-contract=off", "-std=c++20", "-pthread", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1800)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN.replace("%%", "%"))
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2500:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["records"]) > 150 and int(f["deferred_tracebacks"]) > 20 and int(f["multi_best"]) > 3, out.stdout

@@ -5,24 +5,7 @@
   * `select_kernel` (a warp advances std::mt19937(11) 624 outputs at a time and replays the reservoir sampling with libstdc++'s
     Lemire uniform_int_distribution, 32 draws per step) against std::mt19937 + std::uniform_int_distribution themselves — the
     reference's own generator (mapping_generator.h:199-214, chromap.h:863)."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __launch_bounds__(...)
-#define __ldg(p) (*(p))
-#define CTA_NT 128
-static u64 *g_dyn_smem = nullptr;
-static inline void atomicAdd(u64 *p, u64 v) { __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline void agg_add(u64 *addr, u64 v) { atomicAdd(addr, v); }
-'''
+from tests import emu
 
 MAIN = r'''
 #include <cstdio>
@@ -125,35 +108,8 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_pairing_kernels_and_multimapper_sampling(tmp_path):
-    d = open(os.path.join(ROOT, "chromap_b200", "csrc", "device_common.cuh")).read()
-    k = open(os.path.join(ROOT, "chromap_b200", "csrc", "pipeline_kernels.cuh")).read()
-    c = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_pair_candidates.cuh")).read()
-    v = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_verify_pairing.cuh")).read()
-    d = re.sub(r'asm volatile\(.*?\)\s*;', ';', d.replace("#include <cuda_runtime.h>", ""))
-    parts = [d,
-             _between(k, "struct Counters", "// Counter updates: every lane adds to the same address"),
-             _between(k, "struct Tally { int min_err", "// K3: per read — GenerateDraftMappings"),
-             _between(k, "template <typename Visit>\n__device__ __forceinline__ void pair_sweep(", "__global__ void __launch_bounds__(128) select_kernel("),
-             _between(k, "__global__ void __launch_bounds__(128) select_kernel(", "// ------------------------------------------------------------------------------------------------\n// alignment.cc:656-718"),
-             _between(k, "// same for (key, tag) pairs under `less`", "// candidate_processor.cc:283-342 with the sorted hits streamed"),
-             _between(c, "// ---- CTA-wide scans (one value per thread)", "// ---- MergeCandidates (candidate_processor.cc:345-414)"),
-             _between(v, "// Tally (min, #min, second distinct min, #second) of a multiset", "// GenerateDraftMappings for one read (non-split)."),
-             _between(v, "// Best-pair statistics for one pair by one CTA", "// Record emit for one pair of the overflow tiers by one CTA")]
-    body = re.sub(r"#pragma unroll[^\n]*", "", "\n".join(parts)).replace("#pragma once", "")
-    body = body.replace("extern __shared__ u64 smk[];", "u64 *smk = g_dyn_smem;")
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + body + MAIN.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1800)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN.replace("%%", "%"))
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2000:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["with_best"]) > 40 and int(f["sampled_pairs"]) > 300, out.stdout

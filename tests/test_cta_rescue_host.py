@@ -5,19 +5,7 @@ UNCHANGED on the host (tests/cta_emu.h emulates the CTA) against the oracle's li
 (`orc_rescue_test`; the same code the oracle's mapper runs, pinned to the reference binary by tests/test_oracle_golden.py).
 What the reference emits depends on where its binary search happens to stop, window after window; the inputs therefore put
 windows before, inside, between and exactly on occurrence positions, merge neighbouring windows, and include both bail-outs."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __ldg(p) (*(p))
-static inline int atomicAdd(int *p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-'''
+from tests import emu
 
 MAIN = r'''
 #include <cstdio>
@@ -122,31 +110,8 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_both_device_forms_of_the_mate_guided_lookup_equal_the_oracle(tmp_path):
-    d = open(os.path.join(ROOT, "chromap_b200", "csrc", "device_common.cuh")).read()
-    k = open(os.path.join(ROOT, "chromap_b200", "csrc", "pipeline_kernels.cuh")).read()
-    c = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_pair_candidates.cuh")).read()
-    d = d.replace("#include <cuda_runtime.h>", "")
-    d = re.sub(r'asm volatile\(.*?\)\s*;', ';', d)
-    parts = [d,
-             _between(k, "struct RepStats", "// candidate_processor.cc:283-342 — clustering scan"),
-             _between(k, "// index.cc:351-489 — mate-guided lookup on one strand for one read (by one thread).", "// candidate_processor.cc:345-414 — merge c2 into c1"),
-             _between(k, "// ascending bitonic sort of n keys", "// same for (key, tag) pairs under `less`"),
-             _between(c, "// ---- CTA-wide scans (one value per thread)", "// ---- MergeCandidates (candidate_processor.cc:345-414)"),
-             _between(c, "#define RESCUE_MAXWIN 300", "// ---- the kernel ----")]
-    body = "\n".join(parts).replace("#pragma unroll", "").replace("#pragma once", "")
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + body + MAIN.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1800)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN.replace("%%", "%"))
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-1500:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["hits"]) > 5000 and int(f["bails"]) > 6 and int(f["boundary_windows"]) > 800, out.stdout

@@ -5,10 +5,7 @@
 for element with the sequential formulations the tier-0 kernels use (`merge_cands`, `pe_filter_dir` in pipeline_kernels.cuh,
 which are the ones the GPU stage tests pin to the oracle).  Lists are random with many equal / near-equal positions, several
 reference sequences, counts around the rule's thresholds; block sizes 32 .. 512 as the tiers launch them."""
-import os
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests import emu
 
 MAIN = r'''
 #include <cstdio>
@@ -83,21 +80,8 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_cta_merge_and_pe_filter_equal_the_sequential_sweeps(tmp_path):
-    k = open(os.path.join(ROOT, "chromap_b200", "csrc", "pipeline_kernels.cuh")).read()
-    c = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_pair_candidates.cuh")).read()
-    seq = _between(k, "// candidate_processor.cc:345-414 — merge c2 into c1", "// K2: per pair — SupplementCandidates")
-    par = _between(c, "// ---- CTA-wide scans (one value per thread)", "// ---- mate-guided lookup (index.cc:351-489), cooperatively")
-    src = tmp_path / "t.cc"
-    src.write_text('#include "%s"\n' % os.path.join(ROOT, "tests", "cta_emu.h") + seq.replace("#pragma unroll", "") + par.replace("#pragma unroll", "") + MAIN.replace("%%", "%"))
-    exe = tmp_path / "t"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-o", str(exe), str(src)])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1200)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN.replace("%%", "%"), timeout=1200)
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-1500:] + out.stderr[-500:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["unpaired_flagged"]) > 15, out.stdout   # the unpaired-candidate rule was exercised

@@ -5,21 +5,7 @@ UNCHANGED on the host emulation of a CTA (tests/cta_emu.h):
     (candidate_processor.cc:283-342; the form the tier-0 kernel uses and the GPU stage tests pin to the oracle),
   * `cta_minimizers` (k-mer hashes in parallel, window logic replayed over the seeds; fallback for even k / unusual w / N)
     against the oracle's `orc_minimizers` (minimizer_generator.cc:7-139)."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __ldg(p) (*(p))
-#define CTA_NT 128
-static inline u32 __funnelshift_r(u32 lo, u32 hi, u32 s) { return (u32)((((u64)hi << 32) | lo) >> (s & 31)); }
-'''
+from tests import emu
 
 MAIN = r'''
 #include <cstdio>
@@ -107,26 +93,6 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_cta_sorts_clustering_and_minimizers(tmp_path):
-    d = open(os.path.join(ROOT, "chromap_b200", "csrc", "device_common.cuh")).read()
-    m = open(os.path.join(ROOT, "chromap_b200", "csrc", "minimizers.cuh")).read()
-    k = open(os.path.join(ROOT, "chromap_b200", "csrc", "pipeline_kernels.cuh")).read()
-    d = re.sub(r'asm volatile\(.*?\)\s*;', ';', d.replace("#include <cuda_runtime.h>", ""))
-    m = _between(m, "// ---- minimizers ---", "// ---- lane-interleaved minimizer records of tier 0")
-    parts = [d, m,
-             _between(k, "// candidate_processor.cc:283-342 — clustering scan over sorted hits", "// K1c: per read — hit lists from the probed values"),
-             _between(k, "// ascending bitonic sort of n keys", "// S0: tier 0's scratch.")]
-    body = re.sub(r"#pragma unroll[^\n]*", "", "\n".join(parts)).replace("#pragma once", "")
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + body + MAIN.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1800)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN.replace("%%", "%"))
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-1500:] + out.stderr[-800:]

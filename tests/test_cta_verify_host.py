@@ -7,24 +7,7 @@ the code the oracle's mapper runs, pinned to the reference binary by tests/test_
 copies with 0 .. e + 3 edits so that whole groups pass, whole groups fail and groups fail in part; candidates off both ends of
 the reference; single-candidate reads for the fast path; block sizes 128 and 256 as the tiers launch them; e = 4 (8 lanes) and
 e = 8 (4 lanes)."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __launch_bounds__(...)
-#define __ldg(p) (*(p))
-static u64 *g_dyn_smem = nullptr;
-static inline void atomicAdd(u64 *p, u64 v) { __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline void agg_add(u64 *addr, u64 v) { atomicAdd(addr, v); }   // (the device version first adds up the converged lanes)
-static inline int agg_append(int *count) { return __atomic_fetch_add(count, 1, __ATOMIC_RELAXED); }
-'''
+from tests import emu
 
 MAIN = r'''
 #include <cstdio>
@@ -146,32 +129,8 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_verify_cta_kernel_equals_the_oracles_draft_mapping_generation(tmp_path):
-    d = open(os.path.join(ROOT, "chromap_b200", "csrc", "device_common.cuh")).read()
-    k = open(os.path.join(ROOT, "chromap_b200", "csrc", "pipeline_kernels.cuh")).read()
-    c = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_pair_candidates.cuh")).read()
-    v = open(os.path.join(ROOT, "chromap_b200", "csrc", "cta_verify_pairing.cuh")).read()
-    d = re.sub(r'asm volatile\(.*?\)\s*;', ';', d.replace("#include <cuda_runtime.h>", ""))
-    parts = [d,
-             _between(k, "struct Counters", "// Counter updates: every lane adds to the same address"),
-             _between(k, "struct PatPlanes", "// ------------------------------------------------------------------------------------------------\n// mapping_generator.h:346-484 (non-split): two-pointer sweep"),
-             _between(k, "// same for (key, tag) pairs under `less`", "// candidate_processor.cc:283-342 with the sorted hits streamed"),
-             _between(c, "// ---- CTA-wide scans (one value per thread)", "// ---- MergeCandidates (candidate_processor.cc:345-414)"),
-             _between(v, "// Tally (min, #min, second distinct min, #second) of a multiset", "// Best-pair statistics for one pair by one CTA")]
-    body = re.sub(r"#pragma unroll[^\n]*", "", "\n".join(parts)).replace("#pragma once", "")
-    body = body.replace("extern __shared__ u64 smk[];", "u64 *smk = g_dyn_smem;").replace("extern __shared__ u8 v_codes[];", "u8 *v_codes = (u8 *)g_dyn_smem;")
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + body + MAIN.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1800)
+    out = emu.run(tmp_path, emu.PIPELINE, MAIN.replace("%%", "%"))
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2000:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["single_candidate"]) >= 6 and int(f["group_rule"]) > 60 and int(f["mappings"]) > 600, out.stdout

@@ -5,27 +5,7 @@ khash upload kernels `khash_count_kernel` / `khash_insert_kernel`) run UNCHANGED
 (Index::Construct, index.cc:12-89; shown equal to `chromap -i` by tests/test_oracle_golden.py): every key with its singleton
 flag and value, occurrence offsets and counts, the occurrence table entry by entry.  References with N runs, soft-masked
 bases, sequences shorter than a chunk and shorter than k, lengths off the chunk grid, tandem repeats, planted copies; three (k, w)."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-#include <cstring>
-#include <cstdio>
-#include <cstdlib>
-#include <random>
-#include <string>
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __launch_bounds__(...)
-#define __ldg(p) (*(p))
-static inline unsigned long long atomicAdd(unsigned long long *p, unsigned long long v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline unsigned long long atomicCAS(unsigned long long *p, unsigned long long cmp, unsigned long long val) { __atomic_compare_exchange_n(p, &cmp, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED); return cmp; }
-'''
+from tests import emu
 
 MAIN = r'''
 extern "C" {
@@ -131,20 +111,7 @@ int main() {
 
 
 def test_index_build_kernels_equal_the_oracles_index(tmp_path):
-    src_dir = os.path.join(ROOT, "chromap_b200", "csrc")
-    text = "\n".join(open(os.path.join(src_dir, f)).read() for f in ["device_common.cuh", "index_build.cuh"])
-    text = text[:text.index("#define IB_CU(call)")]      # the kernels; build_index_on_device itself is CUDA host code
-    text = re.sub(r'#include [<"][^\n]*', "", text).replace("#pragma once", "")
-    text = re.sub(r'asm volatile\(.*?\)\s*;', ';', text)
-    text = re.sub(r"#pragma unroll[^\n]*", "", text)
-    main = MAIN % dict(orc_h=os.path.join(ROOT, "oracle", "oracle_chromap.h"))
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + "#include <algorithm>\n#include <vector>\n" + text + main.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-w", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1200)
+    out = emu.run(tmp_path, ["device_common.cuh", "index_build.cuh"], MAIN % dict(orc_h=emu.ORACLE_H), timeout=1200)
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2500:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["keys"]) > 50000 and int(f["occurrences"]) > 5000, out.stdout

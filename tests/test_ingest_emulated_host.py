@@ -5,26 +5,8 @@ bases and qualities of every record for LF and CRLF files, names with comments, 
 input that is not plain 4-line FASTQ (a header without '@', a separator without '+', an empty read, quality and sequence of
 different lengths) that send the caller to the host reader."""
 import os
-import re
-import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-#include <cstring>
-#include <cstdio>
-#include <cstdlib>
-#include <random>
-#include <string>
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __ldg(p) (*(p))
-static inline u32 atomicAdd(u32 *p, u32 v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline u32 atomicMin(u32 *p, u32 v) { u32 o = *p; if (v < o) *p = v; return o; }   // (serial emulation)
-static inline u32 atomicMax(u32 *p, u32 v) { u32 o = *p; if (v > o) *p = v; return o; }
-'''
+from tests import emu
 
 MAIN = r'''
 #include "%(seqio_h)s"
@@ -109,16 +91,9 @@ int main(int argc, char **argv) {
 
 
 def test_fastq_ingest_kernels_equal_the_host_reader(tmp_path):
-    src_dir = os.path.join(ROOT, "chromap_b200", "csrc")
-    text = "\n".join(open(os.path.join(src_dir, f)).read() for f in ["device_common.cuh", "ingest.cuh"])
-    text = re.sub(r'#include [<"][^\n]*', "", text).replace("#pragma once", "")
-    text = re.sub(r'asm volatile\(.*?\)\s*;', ';', text)
-    main = MAIN % dict(seqio_h=os.path.join(src_dir, "host", "seqio.h"))
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + "#include <algorithm>\n#include <vector>\n" + text + main.replace("%%", "%"))
-    exe = tmp_path / "t"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-w", "-o", str(exe), str(src), os.path.join(src_dir, "host", "seqio.cc"), "-lz"])
-    out = subprocess.run([str(exe), str(tmp_path)], capture_output=True, text=True, timeout=1200)
+    host = os.path.join(emu.CSRC, "host")
+    out = emu.run(tmp_path, ["device_common.cuh", "ingest.cuh"], MAIN % dict(seqio_h=os.path.join(host, "seqio.h")), args=[str(tmp_path)], timeout=1200,
+                  sources=[os.path.join(host, "seqio.cc")], libs=["-lz"])
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2500:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["records"]) > 5000 and int(f["defective_files"]) > 20, out.stdout

@@ -2,26 +2,9 @@
 tier-0 front end) compiled for the HOST and compared with each other on random, low-complexity, tandem-repeat and N-bearing
 reads.  (The run-time body is compared with the oracle on the GPU by the stage tests; this keeps the fast paths honest on
 machines without one.)"""
-import os
-import re
-import subprocess
+from tests import emu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''#include <cstdio>
-#include <cstdint>
-#include <cstdlib>
-#include <vector>
-#include <algorithm>
-#include <string>
-typedef unsigned long long u64; typedef unsigned int u32; typedef unsigned char u8;
-#define CMX_W_MAX 64
-using std::min; using std::max;
-static inline u32 __funnelshift_r(u32 lo,u32 hi,u32 s){ return (u32)((((u64)hi<<32)|lo)>>(s&31)); }
-static inline u32 base_code(u8 c){ switch(c){case 'A':case 'a':return 0;case 'C':case 'c':return 1;case 'G':case 'g':return 2;case 'T':case 't':return 3;default:return 4;} }
-static inline u64 mix64(u64 key,u64 mask){ key = (~key + (key << 21)) & mask; key = key ^ key >> 24; key = ((key + (key << 3)) + (key << 8)) & mask; key = key ^ key >> 14; key = ((key + (key << 2)) + (key << 4)) & mask; key = key ^ key >> 28; key = (key + (key << 31)) & mask; return key;}
-'''
-POST = r'''
+MAIN = r'''
 int main(){
   srand(5); long bad=0, tot=0, ties=0;
   // Hash64 on 32-bit halves == the 64-bit formulation
@@ -52,14 +35,6 @@ int main(){
 
 
 def test_minimizer_scans_agree_on_the_host(tmp_path):
-    s = open(os.path.join(ROOT, "chromap_b200", "csrc", "minimizers.cuh")).read()
-    s = s[:s.index("// ---- lane-interleaved minimizer records of tier 0")]
-    s = s.replace('#include "device_common.cuh"', "").replace("#pragma once", "").replace("__device__ __forceinline__", "static inline")
-    s = re.sub(r"#pragma unroll[^\n]*", "", s)
-    src = tmp_path / "t.cc"
-    src.write_text(PRE + s + POST)
-    exe = tmp_path / "t"
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-o", str(exe), str(src)])
-    out = subprocess.run([str(exe)], capture_output=True, text=True)
+    out = emu.run(tmp_path, ["device_common.cuh", "minimizers.cuh"], MAIN)
     assert out.returncode == 0, out.stdout
     assert "bad=0" in out.stdout and "ties=0" not in out.stdout, out.stdout

@@ -3,12 +3,12 @@ seed_cta -> pair_candidates_cta -> verify_cta -> pairing_cta (overflow tiers, on
 between the tiers, select, emit (+ deferred tracebacks) / emit_cta — compiled from the UNCHANGED kernel sources
 (device_common.cuh, minimizers.cuh, pipeline_kernels.cuh, seed_front.cuh, cta_pair_candidates.cuh, cta_verify_pairing.cuh, sam_kernels.cuh) and run on the host
 emulation of CTAs (tests/cta_emu.h) with the launch sequence, grid / block sizes, shared-memory sizes and scratch layout of
-api.cu's run_lane (the layout code itself is cut out of api.cu), against the oracle's mapper (`orc_map_pairs`, pinned to the
+the library's run_lane (the layout by the library's own `scratch_layout`), against the oracle's mapper (`orc_map_pairs`, pinned to the
 reference binary by tests/test_oracle_golden.py): every pair's records, field by field.
 The front end runs too (seed_front_kernel: persistent grid, double-buffered read tiles, packed-key minimizer scan, table probes,
-lane-interleaved records): only its six PTX wrappers (mbarrier.* / cp.async.bulk) are replaced by host equivalents — an mbarrier
-word with byte and arrival counts, a copy that signals its bytes — and its records are also compared one by one with the
-oracle's minimizers and khash lookups.
+lane-interleaved records): only its six PTX wrappers (mbarrier.* / cp.async.bulk) are replaced by cta_emu.h's host equivalents —
+an mbarrier word with byte and arrival counts, a copy that signals its bytes — and its records are also compared one by one with
+the oracle's minimizers and khash lookups.
 Runs: `--preset chip` with the real tier capacities (64 / 32 / 32 ...) on a reference with repeat families, reads longer than the first tier
 allows, N's and junk pairs; and tiny first- and second-tier capacities that push most ordinary pairs through the CTA kernels and
 some of them up to the last tier (512-thread pair_candidates_cta, 256-thread verify_cta), with -n 3; `--preset atac` (adapter
@@ -20,70 +20,12 @@ import os
 import re
 import subprocess
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-#include <cmath>
-#include <cstring>
-#include <cstdio>
-#include <cstdlib>
-#include <random>
-#include <string>
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __launch_bounds__(...)
-#define __noinline__
-#define __ldg(p) (*(p))
-static u64 *g_dyn_smem = nullptr;
-static inline u64 atomicAdd(u64 *p, u64 v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline int atomicAdd(int *p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline u32 atomicAdd(u32 *p, u32 v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
-static inline int atomicExch(int *p, int v) { return __atomic_exchange_n(p, v, __ATOMIC_RELAXED); }
-static inline u64 atomicCAS(u64 *p, u64 cmp, u64 val) { __atomic_compare_exchange_n(p, &cmp, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED); return cmp; }
-static inline void agg_add(u64 *addr, u64 v) { atomicAdd(addr, v); }     // (device: one atomic per group of converged lanes)
-static inline int agg_append(int *count) { return atomicAdd(count, 1); }
-static inline double __dmul_rn(double a, double b) { return a * b; }
-static inline double __dadd_rn(double a, double b) { return a + b; }
-static inline double __ddiv_rn(double a, double b) { return a / b; }
-static inline double __dsqrt_rn(double a) { return std::sqrt(a); }
-static inline u32 __funnelshift_r(u32 lo, u32 hi, u32 s) { return (u32)((((u64)hi << 32) | lo) >> (s & 31)); }
-// ---- host equivalents of seed_front.cuh's six PTX wrappers (mbarrier + cp.async.bulk); everything else of that file is compiled as it is.
-// An mbarrier word: bits 0-31 = bytes still expected, bits 32-47 = arrivals still expected, bits 48-63 = completed phases.  The
-// "copy engine" copies at issue time and then signals its bytes, like complete_tx.
-#include <sched.h>
-static inline void emu_mbar_settle(u64 *bar) {   // a phase completes when no arrival and no byte is outstanding: re-arm with one arrival
-  u64 v = __atomic_load_n(bar, __ATOMIC_ACQUIRE);
-  if ((v & 0xFFFFFFFFFFFFull) == 0) __atomic_store_n(bar, ((v >> 48) + 1) << 48 | (1ull << 32), __ATOMIC_RELEASE);
-}
-static inline u32 smem_u32(const void *p) { return (u32)(size_t)p; }
-static inline void mbar_init(u64 *bar, u32 count) { __atomic_store_n(bar, (u64)count << 32, __ATOMIC_RELEASE); }
-static inline void mbar_fence_init() {}
-static inline void mbar_arrive_expect_tx(u64 *bar, u32 bytes) {   // (called by one thread, before its copies)
-  u64 v = __atomic_load_n(bar, __ATOMIC_ACQUIRE);
-  v = (v & 0xFFFF000000000000ull) | ((((v >> 32) & 0xFFFF) - 1) << 32) | (u64)((u32)v + bytes);
-  __atomic_store_n(bar, v, __ATOMIC_RELEASE);
-  emu_mbar_settle(bar);
-}
-static inline bool mbar_try_wait(u64 *bar, u32 parity) {
-  const bool done = (((__atomic_load_n(bar, __ATOMIC_ACQUIRE) >> 48) & 1u) != parity);
-  if (!done) sched_yield();
-  return done;
-}
-static inline void bulk_g2s(void *dst, const void *src, u32 bytes, u64 *bar) {
-  memcpy(dst, src, bytes);
-  u64 v = __atomic_load_n(bar, __ATOMIC_ACQUIRE);
-  __atomic_store_n(bar, (v & 0xFFFFFFFF00000000ull) | (u64)((u32)v - bytes), __ATOMIC_RELEASE);
-  emu_mbar_settle(bar);
-}
-'''
+from tests import emu
 
 MAIN = r'''
 extern "C" {
 #include "%(orc_h)s"
 }
-%(tier_bytes)s
 struct HostTier {
   Caps caps;
   std::vector<char> mem;
@@ -92,27 +34,20 @@ struct HostTier {
   std::vector<int> list;   // pair list of this tier (empty = identity)
 };
 static void tier_prepare_host(HostTier &t, int n_slots, const int *pair_list, bool interleaved) {
-  size_t o[11];
-  const size_t bytes = tier_bytes(t.caps, (size_t)n_slots + 1, interleaved, o);
+  size_t o[SCRATCH_ARRAYS];
+  const size_t bytes = scratch_layout(t.caps, (size_t)n_slots + 1, interleaved, o);
   t.mem.assign(bytes + 256, (char)0x5A);   // (scratch is not cleared on the device either)
-  char *b = t.mem.data();
+  char *a[SCRATCH_ARRAYS];
+  for (int i = 0; i < SCRATCH_ARRAYS; ++i) a[i] = t.mem.data() + o[i];
+  if (getenv("EMU_EXACT_SCRATCH")) {
+    size_t sz[SCRATCH_ARRAYS];
+    scratch_layout(t.caps, (size_t)n_slots, interleaved, o, sz);
+    t.parts.assign(SCRATCH_ARRAYS, std::vector<char>());
+    for (int i = 0; i < SCRATCH_ARRAYS; ++i) { t.parts[(size_t)i].assign(sz[i] ? sz[i] : 8, (char)0x5A); a[i] = t.parts[(size_t)i].data(); }
+  }
   Scratch &S = t.view;
   S.caps = t.caps; S.n_slots = n_slots; S.pair_list = pair_list; S.mm_il = interleaved ? 1 : 0;
-  S.rmeta = (ReadMeta *)(b + o[0]); S.pmeta = (PairMeta *)(b + o[1]);
-  S.mm_hash = (u64 *)(b + o[2]); S.mm_val = (u64 *)(b + o[3]); S.mm_pos = (u32 *)(b + o[4]);
-  S.hits = (u64 *)(b + o[5]); S.cand_pos = (u64 *)(b + o[6]); S.cand_cnt = (u8 *)(b + o[7]);
-  S.map_pos = (u64 *)(b + o[8]); S.map_err = (short *)(b + o[9]); S.map_split = (int *)(b + o[10]);
-  if (getenv("EMU_EXACT_SCRATCH")) {
-    const Caps &c = t.caps;
-    const size_t slots = (size_t)n_slots, R = 2 * slots, Rm = interleaved ? 2 * ((slots + 31) / 32 * 32) : R;
-    const size_t sz[11] = {R * sizeof(ReadMeta), slots * sizeof(PairMeta), interleaved ? 0 : R * c.maxmm * 8, Rm * c.maxmm * 8, Rm * c.maxmm * 4, R * 2 * (size_t)c.hc * 8,
-                           R * 6 * (size_t)c.cc * 8, R * 6 * (size_t)c.cc, R * 2 * (size_t)c.mc * 8, R * 2 * (size_t)c.mc * 2, R * 2 * (size_t)c.mc * 4};
-    t.parts.assign(11, std::vector<char>());
-    for (int i = 0; i < 11; ++i) t.parts[(size_t)i].assign(sz[i] ? sz[i] : 8, (char)0x5A);
-    S.rmeta = (ReadMeta *)t.parts[0].data(); S.pmeta = (PairMeta *)t.parts[1].data(); S.mm_hash = (u64 *)t.parts[2].data(); S.mm_val = (u64 *)t.parts[3].data();
-    S.mm_pos = (u32 *)t.parts[4].data(); S.hits = (u64 *)t.parts[5].data(); S.cand_pos = (u64 *)t.parts[6].data(); S.cand_cnt = (u8 *)t.parts[7].data();
-    S.map_pos = (u64 *)t.parts[8].data(); S.map_err = (short *)t.parts[9].data(); S.map_split = (int *)t.parts[10].data();
-  }
+  scratch_bind(S, a);
 }
 static std::vector<u64> g_smem;
 template <typename F>
@@ -227,11 +162,8 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   DevRef R{(const u8 *)refmem.data(), roff, rlen, 2};
   DevBatch B{};
   B.seq1 = (const u8 *)s1.data(); B.off1 = o1.data(); B.seq2 = (const u8 *)s2.data(); B.off2 = o2.data(); B.n_pairs = (u32)n; B.first_read_id = first_read_id;
-  std::vector<double> il_; std::vector<int> thr_;
-  {
-%(tables)s
-    il_ = il; thr_ = thr;
-  }
+  std::vector<double> il_(65536); std::vector<int> thr_(96);
+  mapq_tables_fill(il_.data(), thr_.data());
   MapqTables T{il_.data(), thr_.data()};
   u32 mt_init[624];
   mt_init[0] = 11u;
@@ -400,7 +332,7 @@ int main() {
   static_assert(sizeof(OutRecord) == sizeof(orc_pe_record) && sizeof(OutPairs) == sizeof(orc_pe_record), "record layouts");
   long bad = 0;
   const int mrl = 80;
-  const Caps real[3] = {{mrl, 64, 32, 32}, {mrl * 2, 1024, 256, 256}, {mrl * 4, 65536, 8192, 8192}};   // api.cu's tiers
+  const Caps real[3] = {{mrl, 64, 32, 32}, {mrl * 2, 1024, 256, 256}, {mrl * 4, 65536, 8192, 8192}};   // the library's tiers
   const Caps small[3] = {{mrl, 6, 2, 2}, {mrl * 2, 40, 6, 6}, {mrl * 4, 65536, 8192, 8192}};            // most pairs through the CTA kernels, some to the last tier
   const Caps real_long[3] = {{150, 64, 32, 32}, {300, 1024, 256, 256}, {600, 65536, 8192, 8192}};
   const Caps small_long[3] = {{150, 6, 2, 2}, {300, 40, 6, 6}, {600, 65536, 8192, 8192}};
@@ -432,43 +364,13 @@ int main() {
 '''
 
 
-def _between(s, a, b):
-    i = s.index(a)
-    return s[i:s.index(b, i)]
-
-
 def test_device_pipeline_on_emulated_ctas_equals_the_oracle(tmp_path):
-    src_dir = os.path.join(ROOT, "chromap_b200", "csrc")
-    files = ["device_common.cuh", "minimizers.cuh", "pipeline_kernels.cuh", "seed_front.cuh", "cta_pair_candidates.cuh", "cta_verify_pairing.cuh", "sam_kernels.cuh"]
-    text = "\n".join(open(os.path.join(src_dir, f)).read() for f in files).replace("#ifdef __CUDACC__", "#if 1")
-    # seed_front.cuh's six PTX wrappers (mbarrier, cp.async.bulk) are the only device code replaced: host equivalents in PRE
-    a = text.index("// ---- mbarrier + bulk copy (PTX ISA 8.x, sm_90+)")
-    b = text.index("// ---- the kernel ------", a)
-    text = text[:a] + text[b:]
-    text = text.replace("extern __shared__ __align__(16) u8 sf_smem[];", "u8 *sf_smem = (u8 *)g_dyn_smem;")
-    api = open(os.path.join(src_dir, "api.cu")).read()
-    text = re.sub(r'#include [<"][^\n]*', "", text).replace("#pragma once", "")
-    text = re.sub(r'asm volatile\(.*?\)\s*;', ';', text)
-    text = re.sub(r"#pragma unroll[^\n]*", "", text)
-    text = re.sub(r"extern __shared__ (\w+) (\w+)\[\];", r"\1 *\2 = (\1 *)g_dyn_smem;", text)
-    # the two counter helpers use __activemask: the harness supplies plain atomics instead
-    a = text.index("// Counter updates: every lane adds to the same address")
-    b = text.index("// ------------------------------------------------------------------------------------------------\n// K0: per pair")
-    text = text[:a] + text[b:]
-    tables = _between(api, "    std::vector<double> il(65536, 0.0);", "    CUC(cudaMalloc(&ctx->inv_log")
-    tier_bytes = _between(api, "static size_t tier_bytes(", "static cudaError_t tier_prepare(")
-    main = MAIN % dict(orc_h=os.path.join(ROOT, "oracle", "oracle_chromap.h"), tier_bytes=tier_bytes.replace("%", "%%"), tables=tables.replace("%", "%%"))
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + text + main.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
     # CMX_EMU_SANITIZE=address | thread: the same run under AddressSanitizer (out-of-bounds accesses of reads, reference, table,
     # occurrence lists, shared memory) or ThreadSanitizer (the emulation's answer to racecheck: a missing __syncthreads between two
     # phases of a kernel is a data race between the OS threads that play the CUDA threads).  Minutes instead of seconds: on request.
     san = os.environ.get("CMX_EMU_SANITIZE", "")
     flags = ["-fsanitize=" + san, "-g", "-fno-omit-frame-pointer"] if san in ("address", "thread") else []
-    subprocess.check_call(["g++", "-O1", "-ffp-contract=off", "-std=c++20", "-pthread", "-w"] + flags + ["-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
+    exe = emu.build(tmp_path, emu.PIPELINE, MAIN % dict(orc_h=emu.ORACLE_H), flags=flags)
     if san == "address":
         os.environ["EMU_EXACT_SCRATCH"] = "1"
     env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0", TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0 exitcode=0")

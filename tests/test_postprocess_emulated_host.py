@@ -3,27 +3,8 @@ heads, survivor rule) and the kernels of the multi-GPU duplicate removal (exchan
 rule, gather; the range shuffle's key / sample / destination / bucket-bound kernels) and the BED text kernels run UNCHANGED on the host emulation
 (tests/cta_emu.h) against the oracle's post-processing (`orc_postprocess`, `_bc`, `_pairs`, `_se`; mapping_processor.h:100-202,
 mapping_writer.h:166-376, pinned to the reference binary by the golden BED / pairs files).  The library drives these kernels
-with CUB's stable LSD radix passes (api.cu); here std::stable_sort plays CUB, in the same pass order."""
-import os
-import re
-import subprocess
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-PRE = r'''
-#include "%(emu)s"
-#include <cstring>
-#include <cstdio>
-#include <cstdlib>
-#include <numeric>
-#include <random>
-struct ulonglong2 { u64 x, y; };
-#define __host__
-#define __shared__ static
-#define __launch_bounds__(...)
-#define __ldg(p) (*(p))
-static inline u64 atomicMax(unsigned long long *p, unsigned long long v) { u64 o = __atomic_load_n(p, __ATOMIC_RELAXED); while (o < v && !__atomic_compare_exchange_n(p, &o, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return o; }
-'''
+with CUB's stable LSD radix passes (pp_device); here std::stable_sort plays CUB, in the same pass order."""
+from tests import emu
 
 MAIN = r'''
 extern "C" {
@@ -64,7 +45,7 @@ int main() {
   // ---- postprocess.cuh against the oracle
   for (int kind : {PP_BED, PP_BED_BC, PP_PAIRS, PP_BED_SE})
     for (int low_mem = 0; low_mem < 2; ++low_mem) for (int dedup = 0; dedup < 2; ++dedup) for (int tn5 = 0; tn5 < 2; ++tn5) for (int q : {0, 30}) {
-      if (kind == PP_PAIRS && (tn5 || (dedup && !low_mem))) continue;     // pairs: no Tn5; duplicate removal only with the low-memory rule (api.cu refuses the other)
+      if (kind == PP_PAIRS && (tn5 || (dedup && !low_mem))) continue;     // pairs: no Tn5; duplicate removal only with the low-memory rule (the library refuses the other)
       const size_t n = 3000;
       std::vector<PpRecord> recs = random_records(g, n, kind);
       std::vector<u64> bcs(n);
@@ -79,7 +60,7 @@ int main() {
       const long nw = kind == PP_PAIRS ? (long)orc_postprocess_pairs(&op, (orc_pairs_record *)want.data(), (long)n)
                       : bc ? (long)orc_postprocess_bc(&op, (orc_pe_record *)want.data(), (uint64_t *)wbc.data(), (long)n)
                       : kind == PP_BED_SE ? (long)orc_postprocess_se(&op, (orc_pe_record *)want.data(), (long)n) : (long)orc_postprocess(&op, (orc_pe_record *)want.data(), (long)n);
-      // pp_device's sequence (api.cu), std::stable_sort in CUB's place
+      // pp_device's sequence, std::stable_sort in CUB's place
       std::vector<PpRecord> a = recs, b2(n), res(n);
       std::vector<u64> bca = bcs, bcb(n), resbc(n), keys(n);
       std::vector<u32> idx(n);
@@ -230,20 +211,7 @@ int main() {
 
 
 def test_postprocess_and_exchange_kernels_equal_the_oracle(tmp_path):
-    src_dir = os.path.join(ROOT, "chromap_b200", "csrc")
-    files = ["device_common.cuh", "postprocess.cuh", "exchange.cuh"]
-    text = "\n".join(open(os.path.join(src_dir, f)).read() for f in files)
-    text = re.sub(r'#include [<"][^\n]*', "", text).replace("#pragma once", "")
-    text = re.sub(r'asm volatile\(.*?\)\s*;', ';', text)
-    text = re.sub(r"#pragma unroll[^\n]*", "", text)
-    main = MAIN % dict(orc_h=os.path.join(ROOT, "oracle", "oracle_chromap.h"))
-    src = tmp_path / "t.cc"
-    src.write_text(PRE % dict(emu=os.path.join(ROOT, "tests", "cta_emu.h")) + text + main.replace("%%", "%"))
-    exe = tmp_path / "t"
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    assert os.path.exists(lib), "oracle/liboracle.so not built (__graft_entry__.build())"
-    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-w", "-o", str(exe), str(src), lib, "-Wl,-rpath," + os.path.dirname(lib), "-fopenmp"])
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=1200)
+    out = emu.run(tmp_path, ["device_common.cuh", "postprocess.cuh", "exchange.cuh"], MAIN % dict(orc_h=emu.ORACLE_H), timeout=1200)
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2500:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
     assert int(f["cases"]) > 50 and int(f["records_kept"]) > 50000, out.stdout
