@@ -335,8 +335,8 @@ __device__ inline void pair_candidates_cta_pair(const DevParams &P, const DevInd
   PairMeta &pm = S.pmeta[slot];
   if (pm.status != ST_OK) return;
   ReadMeta *rm = S.rmeta + 2 * slot;
-  auto CP = [&](int mate, int set, int strand) { return S.cand_pos + ((((size_t)(2 * slot + mate)) * 3 + set) * 2 + strand) * c.cc; };
-  auto CC = [&](int mate, int set, int strand) { return S.cand_cnt + ((((size_t)(2 * slot + mate)) * 3 + set) * 2 + strand) * c.cc; };
+  auto CP = [&](int mate, int set, int strand) { return S.cand_pos + cand_base(0, c, 2 * slot + mate, set, strand); };
+  auto CC = [&](int mate, int set, int strand) { return S.cand_cnt + cand_base(0, c, 2 * slot + mate, set, strand); };
   if (P.se) {
     const int a1 = rm[0].n_cand[0] + rm[0].n_cand[1];
     __syncthreads();

@@ -73,10 +73,10 @@ __global__ void __launch_bounds__(VERIFY_NT_MAX) verify_cta_kernel(DevParams P, 
   const Caps c = S.caps;
   const u8 *read = read_ptr(B, pair, mate);
   const int L = rm.len, e = P.e;
-  u64 *mp[2] = {S.map_pos + ((size_t)sr * 2 + 0) * c.mc, S.map_pos + ((size_t)sr * 2 + 1) * c.mc};
-  short *me[2] = {S.map_err + ((size_t)sr * 2 + 0) * c.mc, S.map_err + ((size_t)sr * 2 + 1) * c.mc};
-  u64 *cp[2] = {S.cand_pos + (((size_t)sr * 3 + 0) * 2 + 0) * c.cc, S.cand_pos + (((size_t)sr * 3 + 0) * 2 + 1) * c.cc};
-  u8 *cc[2] = {S.cand_cnt + (((size_t)sr * 3 + 0) * 2 + 0) * c.cc, S.cand_cnt + (((size_t)sr * 3 + 0) * 2 + 1) * c.cc};
+  u64 *mp[2] = {S.map_pos + map_base(0, c, sr, 0), S.map_pos + map_base(0, c, sr, 1)};
+  short *me[2] = {S.map_err + map_base(0, c, sr, 0), S.map_err + map_base(0, c, sr, 1)};
+  u64 *cp[2] = {S.cand_pos + cand_base(0, c, sr, 0, 0), S.cand_pos + cand_base(0, c, sr, 0, 1)};
+  u8 *cc[2] = {S.cand_cnt + cand_base(0, c, sr, 0, 0), S.cand_cnt + cand_base(0, c, sr, 0, 1)};
   const int nc[2] = {rm.n_cand[0], rm.n_cand[1]};
   if (nc[0] + nc[1] == 1) {  // fast path (draft_mapping_generator.cc:72-157): the only candidate carries every minimizer
     const int strand = nc[0] == 1 ? 0 : 1;
@@ -257,8 +257,8 @@ __global__ void __launch_bounds__(CTA_NT) pairing_cta_kernel(DevParams P, Scratc
   short *me[2][2];
   for (int m = 0; m < 2; ++m)
     for (int s = 0; s < 2; ++s) {
-      mp[m][s] = S.map_pos + ((size_t)(2 * slot + m) * 2 + s) * c.mc;
-      me[m][s] = S.map_err + ((size_t)(2 * slot + m) * 2 + s) * c.mc;
+      mp[m][s] = S.map_pos + map_base(0, c, 2 * slot + m, s);
+      me[m][s] = S.map_err + map_base(0, c, 2 * slot + m, s);
       cta_sort_pairs<short>(mp[m][s], me[m][s], rm[m].n_map[s], ~0ull, (short)32767, mless, smk, smt, sm_cap);
     }
   const int sentinel = 2 * P.e + 1;
@@ -310,8 +310,8 @@ __global__ void __launch_bounds__(CTA_NT) emit_cta_kernel(DevParams P, DevRef R,
   for (int dir = 0; dir < 2; ++dir) {
     if (base > s_sel[to_report - 1]) break;  // every selected index lies in the directions already walked
     W.s1 = dir;
-    const u64 *p1 = S.map_pos + ((size_t)(2 * slot + 0) * 2 + dir) * c.mc, *p2 = S.map_pos + ((size_t)(2 * slot + 1) * 2 + (1 - dir)) * c.mc;
-    const short *e1 = S.map_err + ((size_t)(2 * slot + 0) * 2 + dir) * c.mc, *e2 = S.map_err + ((size_t)(2 * slot + 1) * 2 + (1 - dir)) * c.mc;
+    const u64 *p1 = S.map_pos + map_base(0, c, 2 * slot, dir), *p2 = S.map_pos + map_base(0, c, 2 * slot + 1, 1 - dir);
+    const short *e1 = S.map_err + map_base(0, c, 2 * slot, dir), *e2 = S.map_err + map_base(0, c, 2 * slot + 1, 1 - dir);
     const int n1 = rm[0].n_map[dir], n2 = rm[1].n_map[1 - dir];
     const int C = (n1 + CTA_NT - 1) / CTA_NT;
     const int r0 = min(n1, tid * C), r1 = min(n1, r0 + C);
@@ -346,7 +346,7 @@ __global__ void __launch_bounds__(CTA_NT) emit_cta_kernel(DevParams P, DevRef R,
   // best pairs exist for every selected index (the selection never exceeds n_best), so all to_report records are reported
   if (tid < to_report) {
     const int s1 = s_i1[tid] >> 30, i1 = s_i1[tid] & 0x3FFFFFFF, j = s_j[tid];
-    const size_t b1 = ((size_t)(2 * slot + 0) * 2 + s1) * c.mc + i1, b2 = ((size_t)(2 * slot + 1) * 2 + (1 - s1)) * c.mc + j;
+    const size_t b1 = map_base(0, c, 2 * slot, s1) + i1, b2 = map_base(0, c, 2 * slot + 1, 1 - s1) + j;
     out[(size_t)pair * mb + tid] = pe_record(P, R, B, T, pm, rm, pair, s1, S.map_pos[b1], S.map_err[b1], S.map_pos[b2], S.map_err[b2]);
   }
   if (tid != 0) return;

@@ -80,13 +80,13 @@ struct Scratch {
   Caps caps;
   int n_slots;
   const int *pair_list;  // slot -> pair index in batch (nullptr = identity)
-  int mm_il;             // 1: minimizer records lane-interleaved in groups of 32 pairs (tier 0), see minimizers.cuh
+  int mm_il;             // 1: the per-read arrays mm_val .. map_split, hits excepted, lane-interleaved in groups of 32 pairs (tier 0), see il_read
   ReadMeta *rmeta;       // [2*n_slots]
   PairMeta *pmeta;       // [n_slots]
   u64 *mm_hash;          // [2n][maxmm]   (overflow tiers only)
   u64 *mm_val;           // [2n][maxmm]   lookup value
   u32 *mm_pos;           // [2n][maxmm]   (pos<<1|strand) | kind<<30   kind: 0 absent 1 singleton 2 multi
-  u64 *hits;             // [2n][2][hc]
+  u64 *hits;             // [2n][2][hc]   (never interleaved)
   u64 *cand_pos;         // [2n][3][2][cc]   set 0 = candidates, 1 = buffer, 2 = augment
   u8 *cand_cnt;          // same shape
   u64 *map_pos;          // [2n][2][mc]
@@ -100,11 +100,11 @@ struct Scratch {
 #define SCRATCH_ARRAYS 11
 inline size_t scratch_layout(const Caps &c, size_t slots, bool interleaved, size_t *off, size_t *size = nullptr) {
   const size_t R = 2 * slots;
-  const size_t Rm = interleaved ? 2 * ((slots + 31) / 32 * 32) : R;  // minimizer records: whole groups of 32 pairs
+  const size_t Ri = interleaved ? 2 * ((slots + 31) / 32 * 32) : R;  // interleaved arrays: whole groups of 32 pairs
   const size_t sz[SCRATCH_ARRAYS] = {R * sizeof(ReadMeta), slots * sizeof(PairMeta),
                                      interleaved ? 0 : R * c.maxmm * 8,  // hashes: tier 0 never stores them
-                                     Rm * c.maxmm * 8, Rm * c.maxmm * 4, R * 2 * (size_t)c.hc * 8, R * 6 * (size_t)c.cc * 8, R * 6 * (size_t)c.cc,
-                                     R * 2 * (size_t)c.mc * 8, R * 2 * (size_t)c.mc * 2, R * 2 * (size_t)c.mc * 4};
+                                     Ri * c.maxmm * 8, Ri * c.maxmm * 4, R * 2 * (size_t)c.hc * 8, Ri * 6 * (size_t)c.cc * 8, Ri * 6 * (size_t)c.cc,
+                                     Ri * 2 * (size_t)c.mc * 8, Ri * 2 * (size_t)c.mc * 2, Ri * 2 * (size_t)c.mc * 4};
   size_t end = 0;
   for (int i = 0; i < SCRATCH_ARRAYS; ++i) {
     off[i] = end;
@@ -119,6 +119,53 @@ inline void scratch_bind(Scratch &S, char *const *a) {
   S.mm_hash = (u64 *)a[2]; S.mm_val = (u64 *)a[3]; S.mm_pos = (u32 *)a[4];
   S.hits = (u64 *)a[5]; S.cand_pos = (u64 *)a[6]; S.cand_cnt = (u8 *)a[7];
   S.map_pos = (u64 *)a[8]; S.map_err = (short *)a[9]; S.map_split = (int *)a[10];
+}
+
+// a[i] view of every `stride`-th element starting at base: a per-thread column of an interleaved shared-memory tile (a
+// negative stride walks it backwards) or one list of a tier's per-read arrays (below).
+template <typename T>
+struct Strided {
+  T *base;
+  int stride;
+  __device__ __forceinline__ T &operator[](int i) const { return base[i * stride]; }
+};
+
+// ---- where the lists of read sr = 2 * slot + mate lie in its tier's scratch: minimizer records [maxmm], candidates
+// [3 sets][2 strands][cc], draft mappings [2 strands][mc].
+// il = 1 (tier 0, S.mm_il): lane-interleaved in groups of 32 pairs.  Row `row` of the read's rows lies at
+// (((slot >> 5) * 2 + mate) * rows + row) * 32 + (slot & 31), one row per element (stride 32): the lanes of a warp hold
+// consecutive slots, so their element i is one contiguous segment instead of one sector per lane.  il = 0 (overflow tiers,
+// one CTA per read or pair): [read][rows], stride 1.  The kernels that run in every tier take il from S.mm_il; the CTA-only
+// kernels pass 0 and keep plain pointers.
+// il_read: the read's row block (its group's mate block when interleaved); il_place: where that row block's element e lies.
+__device__ __forceinline__ size_t il_read(int il, int sr) { return il ? (size_t)((sr >> 6) * 2 + (sr & 1)) : (size_t)sr; }
+__device__ __forceinline__ size_t il_place(int il, int sr, size_t e) { return il ? e * 32 + ((sr >> 1) & 31) : e; }
+__device__ __forceinline__ int il_stride(int il) { return il ? 32 : 1; }
+__device__ __forceinline__ size_t mm_base(const Scratch &S, int slot, int mate) {  // == il_place(il, sr, il_read(il, sr) * maxmm)
+  return S.mm_il ? ((size_t)((slot >> 5) * 2 + mate) * S.caps.maxmm) * 32 + (slot & 31) : (size_t)(2 * slot + mate) * S.caps.maxmm;
+}
+__device__ __forceinline__ int mm_stride(const Scratch &S) { return il_stride(S.mm_il); }
+__device__ __forceinline__ size_t cand_base(int il, const Caps &c, int sr, int set, int strand) {
+  return il_place(il, sr, ((il_read(il, sr) * 3 + set) * 2 + strand) * c.cc);
+}
+__device__ __forceinline__ size_t map_base(int il, const Caps &c, int sr, int strand) {
+  return il_place(il, sr, (il_read(il, sr) * 2 + strand) * c.mc);
+}
+// the same lists as views in S's own layout
+__device__ __forceinline__ Strided<u64> cand_pos_of(const Scratch &S, int sr, int set, int strand) {
+  return {S.cand_pos + cand_base(S.mm_il, S.caps, sr, set, strand), il_stride(S.mm_il)};
+}
+__device__ __forceinline__ Strided<u8> cand_cnt_of(const Scratch &S, int sr, int set, int strand) {
+  return {S.cand_cnt + cand_base(S.mm_il, S.caps, sr, set, strand), il_stride(S.mm_il)};
+}
+__device__ __forceinline__ Strided<u64> map_pos_of(const Scratch &S, int sr, int strand) {
+  return {S.map_pos + map_base(S.mm_il, S.caps, sr, strand), il_stride(S.mm_il)};
+}
+__device__ __forceinline__ Strided<short> map_err_of(const Scratch &S, int sr, int strand) {
+  return {S.map_err + map_base(S.mm_il, S.caps, sr, strand), il_stride(S.mm_il)};
+}
+__device__ __forceinline__ Strided<int> map_split_of(const Scratch &S, int sr, int strand) {
+  return {S.map_split + map_base(S.mm_il, S.caps, sr, strand), il_stride(S.mm_il)};
 }
 
 __device__ __forceinline__ int slot_pair(const Scratch &S, int slot) { return S.pair_list ? S.pair_list[slot] : slot; }
@@ -209,16 +256,8 @@ __device__ __forceinline__ u64 hit_to_candidate(int k, u64 ref_hit, u32 read_pos
   return ((ref_hit >> 33) << 32) | start;
 }
 
-// a[i] view of every `stride`-th u64 starting at base (a per-thread column of an interleaved shared-memory tile;
-// a negative stride walks it backwards).
-struct StridedU64 {
-  u64 *base;
-  int stride;
-  __device__ __forceinline__ u64 &operator[](int i) const { return base[i * stride]; }
-};
-
 // In-place ascending sort of u64 keys by one thread: insertion for short lists, heapsort otherwise.
-// A = u64* or StridedU64.
+// A = u64* or Strided<u64>.
 template <typename A>
 __device__ inline void sort_u64(A a, int n) {
   if (n <= 24) {
@@ -260,9 +299,9 @@ __device__ inline void sort_u64(A a, int n) {
 }
 
 // Sort (key, tag) pairs ascending by `less(ka,ta,kb,tb)` — used for candidates (count desc, pos asc) and
-// draft mappings (pos asc, err asc).  Insertion for short lists, heapsort otherwise.
-template <typename T, typename Less>
-__device__ inline void sort_pairs(u64 *k, T *t, int n, Less less) {
+// draft mappings (pos asc, err asc).  Insertion for short lists, heapsort otherwise.  K / V: pointers or Strided views.
+template <typename T, typename K, typename V, typename Less>
+__device__ inline void sort_pairs(K k, V t, int n, Less less) {
   if (n <= 24) {
     for (int i = 1; i < n; ++i) {
       const u64 kv = k[i];

@@ -277,11 +277,3 @@ __device__ __forceinline__ void minimizer_scan_any(SeqF SEQ, int len, int k, int
   else minimizer_scan<0, 0>(SEQ, len, k, w, EMIT);
 }
 
-// ---- lane-interleaved minimizer records of tier 0 -------------------------------------------------------------------
-// element i of the read (slot, mate): base + i * 32, base = (((slot >> 5) * 2 + mate) * maxmm) * 32 + (slot & 31).
-// The overflow tiers keep [read][i] (stride 1).  S.mm_il tells which.
-__device__ __forceinline__ size_t mm_base(const Scratch &S, int slot, int mate) {
-  return S.mm_il ? ((size_t)((slot >> 5) * 2 + mate) * S.caps.maxmm) * 32 + (slot & 31) : (size_t)(2 * slot + mate) * S.caps.maxmm;
-}
-__device__ __forceinline__ int mm_stride(const Scratch &S) { return S.mm_il ? 32 : 1; }
-

@@ -140,7 +140,6 @@ __global__ void emit_sam_kernel(DevParams P, DevRef R, DevBatch B, MapqTables T,
   const int pair = slot_pair(S, slot);
   if (pm.status == ST_OVERFLOW) return;
   if (pm.status != ST_OK || pm.n_best > P.drop_rep || pm.n_best == 0) { out_n[pair] = 0; return; }
-  const Caps c = S.caps;
   const ReadMeta *rm = S.rmeta + 2 * slot;
   const int mb = P.max_best;
   const int to_report = mb < pm.n_best ? mb : pm.n_best;
@@ -152,8 +151,8 @@ __global__ void emit_sam_kernel(DevParams P, DevRef R, DevBatch B, MapqTables T,
   const u8 *rd[2] = {read_ptr(B, pair, 0), read_ptr(B, pair, 1)};
   for (int dir = 0; dir < 2 && reported != to_report; ++dir) {
     const int s1 = dir, s2 = 1 - dir;
-    const u64 *p1 = S.map_pos + ((size_t)(2 * slot + 0) * 2 + s1) * c.mc, *p2 = S.map_pos + ((size_t)(2 * slot + 1) * 2 + s2) * c.mc;
-    const short *e1 = S.map_err + ((size_t)(2 * slot + 0) * 2 + s1) * c.mc, *e2 = S.map_err + ((size_t)(2 * slot + 1) * 2 + s2) * c.mc;
+    const Strided<u64> p1 = map_pos_of(S, 2 * slot, s1), p2 = map_pos_of(S, 2 * slot + 1, s2);
+    const Strided<short> e1 = map_err_of(S, 2 * slot, s1), e2 = map_err_of(S, 2 * slot + 1, s2);
     pair_sweep_until(P, s1, (u32)L[0], (u32)L[1], p1, e1, rm[0].n_map[s1], p2, e2, rm[1].n_map[s2], [&](int i1, int j, int sum) -> bool {
       if (sum != pm.min_sum) return false;
       if (idx == sel[reported]) {
@@ -190,7 +189,6 @@ __global__ void emit_sam_se_kernel(DevParams P, DevRef R, DevBatch B, MapqTables
   const int pair = slot_pair(S, slot);
   if (pm.status == ST_OVERFLOW) return;
   if (pm.status != ST_OK || pm.n_best == 0) { out_n[pair] = 0; return; }
-  const Caps c = S.caps;
   const ReadMeta &rm = S.rmeta[2 * slot];
   const int mb = P.max_best, e = P.e, L = rm.len;
   const int to_report = mb < rm.n_best ? mb : rm.n_best;
@@ -198,8 +196,8 @@ __global__ void emit_sam_se_kernel(DevParams P, DevRef R, DevBatch B, MapqTables
   const u8 *r = read_ptr(B, pair, 0);
   int idx = 0, reported = 0;
   for (int s = 0; s < 2 && reported != to_report; ++s) {
-    const u64 *mp = S.map_pos + ((size_t)(2 * slot) * 2 + s) * c.mc;
-    const short *me = S.map_err + ((size_t)(2 * slot) * 2 + s) * c.mc;
+    const Strided<u64> mp = map_pos_of(S, 2 * slot, s);
+    const Strided<short> me = map_err_of(S, 2 * slot, s);
     for (int mi = 0; mi < rm.n_map[s]; ++mi) {
       if ((int)me[mi] > rm.min_err) continue;
       if (idx == sel[reported]) {
