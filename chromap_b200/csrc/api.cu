@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <thread>
 #include <tuple>
@@ -19,6 +20,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include "../../include/chromap_b200.h"
+#include "cuda_owners.cuh"
 #include "index_build.cuh"
 #include "pipeline_kernels.cuh"
 #include "seed_front.cuh"
@@ -36,10 +38,7 @@ static_assert(sizeof(OutSam) == sizeof(cmx_sam_record) && sizeof(OutSam) % 4 == 
 
 #define N_TIERS 3
 
-struct DevBuf {  // grow-only device buffer
-  void *p = nullptr;
-  size_t cap = 0;
-};
+using DevBuf = DevMem<>;  // grow-only device buffer (ensure)
 
 struct Tier {
   Caps caps;
@@ -58,14 +57,14 @@ struct Tier {
 #define CMX_MAX_LANES 4
 struct Lane {
   DevBuf rescue_list, verify_list, emit_list, nbest, sel, out_rec, out_n, offs, chunk_start, cub_tmp, bc_key, bc_ok, out_compact, bc_out;
-  Counters *ctr = nullptr;
-  int *d_count = nullptr;
+  DevMem<Counters> ctr;
+  DevMem<int> d_count;
   Tier tiers[N_TIERS];
-  cudaStream_t stream = nullptr, aux[N_TIERS - 1] = {nullptr, nullptr};  // aux: emit of the overflow tiers, beside tier 0's
-  cudaEvent_t ev_fork = nullptr, ev_join[N_TIERS - 1] = {nullptr, nullptr};
-  cudaEvent_t ev[10] = {};
-  cudaEvent_t ev_sub[2] = {};
-  cudaEvent_t ev_done = nullptr;
+  Stream stream, aux[N_TIERS - 1];  // aux: emit of the overflow tiers, beside tier 0's
+  Event ev_fork, ev_join[N_TIERS - 1];
+  // stage timing: a tier's start, front end done (tier 0), seeding, candidates, verification and pairing done; then the
+  // start of selection, the start of emission and the compacted records
+  Event ev_tier, ev_front, ev_seed, ev_pc, ev_ver, ev_pair, ev_select, ev_emit, ev_out;
   u32 p0 = 0, n = 0;  // pair range of the last call
   int tiers_used = 0;
   std::string err;
@@ -74,7 +73,7 @@ struct Lane {
 #define CMX_INGEST_SLOTS 6
 struct IngestSlot {  // buffers of one cmx_ingest_fastq stream (text in, packed reads out)
   DevBuf text, nl, seq_start, qual_start, len, off, seq, qual, spans, tmp, stats, count;
-  cudaStream_t stream = nullptr;
+  Stream stream;
 };
 
 struct cmx_ctx {
@@ -83,48 +82,46 @@ struct cmx_ctx {
   DevParams dp;
   std::string err;
   // reference
-  u8 *ref_seq = nullptr;
-  u64 *ref_off = nullptr;
-  u32 *ref_len = nullptr;
+  DevMem<u8> ref_seq;
+  DevMem<u64> ref_off;
+  DevMem<u32> ref_len;
   u32 n_seq = 0;
-  u64 ref_bytes = 0;
   std::vector<u64> h_ref_off;
   std::vector<u32> h_ref_len;
   // index
-  ulonglong2 *slots = nullptr;
+  DevMem<ulonglong2> slots;
   u64 n_slots = 0;
-  u64 *occ = nullptr;
+  DevMem<u64> occ;
   u32 n_occ = 0;
   u64 n_keys = 0;
   int k = 0, w = 0;
   // scATAC barcode whitelist
-  ulonglong2 *wl_slots = nullptr;
+  DevMem<ulonglong2> wl_slots;
   u64 wl_n_slots = 0, wl_num_sample = 0;
-  double *wl_pow = nullptr;
+  DevMem<double> wl_pow;
   u32 wl_bc_len = 0;
   int wl_err = 1, wl_output_nw = 0, wl_active = 0;
   double wl_prob = 0.9;
   DevBuf bc_seq, bc_qual;
   // mapq tables
-  double *inv_log = nullptr;
-  int *pen_thr = nullptr;
-  u32 *mt_init = nullptr;  // std::mt19937(11) right after seeding
+  DevMem<double> inv_log;
+  DevMem<int> pen_thr;
+  DevMem<u32> mt_init;  // std::mt19937(11) right after seeding
   // per-batch buffers
   DevBuf seq1, off1, seq2, off2, trace;
   Lane lanes[CMX_MAX_LANES];
   IngestSlot ingest[CMX_INGEST_SLOTS];
   int sf_grid = 132;            // persistent grid of the front-end kernel: SMs x resident CTAs (set by cmx_create)
-  int pcw_grid = 132 * 16;      // persistent grid of the warp-per-pair rescue pass of tier 0
   int n_lanes = CMX_MAX_LANES;  // lanes a multi-batch call is cut into (cmx_set_lanes; CMX_LANES overrides the default)
   int last_lanes_used = 0;
-  cudaStream_t stream = nullptr, up_stream = nullptr, down_stream = nullptr;
+  Stream stream, up_stream, down_stream;
   // page-locked staging of h2d_big (allocated at the first big upload, kept: page-locking costs more than the copy)
-  char *stage[2] = {nullptr, nullptr};
-  cudaEvent_t stage_ev[2] = {nullptr, nullptr};
-  cudaStream_t stage_stream = nullptr;
-  std::vector<cudaEvent_t> ev_up;
-  cudaEvent_t ev_bc = nullptr;
-  cudaEvent_t ev[4] = {};
+  PinnedMem stage[2];
+  Event stage_ev[2];
+  Stream stage_stream;
+  std::vector<Event> ev_up;
+  Event ev_bc;
+  Event ev[4];
   cmx_timing timing;
   u32 last_n_pairs = 0;
   // multi-GPU exchange (cmx_comm_init / cmx_dedup_exchange): an NCCL communicator of this context's own
@@ -147,17 +144,7 @@ static int fail(cmx_ctx *c, int code, const char *fmt, ...) {
     if (e_ != cudaSuccess) return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); \
   } while (0)
 
-static cudaError_t ensure(DevBuf &b, size_t bytes) {
-  if (bytes <= b.cap) return cudaSuccess;
-  if (b.p) cudaFree(b.p);
-  b.p = nullptr;
-  b.cap = 0;
-  const size_t want = bytes + bytes / 8 + 256;
-  cudaError_t e = cudaMalloc(&b.p, want);
-  if (e == cudaSuccess) b.cap = want;
-  return e;
-}
-static void release(DevBuf &b) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
+static cudaError_t ensure(DevBuf &b, size_t bytes) { return bytes <= b.cap ? cudaSuccess : b.alloc(bytes + bytes / 8 + 256); }
 
 extern "C" {
 
@@ -194,73 +181,65 @@ int cmx_create(cmx_ctx **out, int device, const cmx_params *params) {
   if (params->batch_size < 1 || params->max_read_length < params->min_read_length) return CMX_ERR_INVALID;
   if (params->single_end && (params->split_alignment || params->output_format == 5)) return CMX_ERR_INVALID;  // single-end: BED / TagAlign only
   if (params->output_format == 5 && params->remove_pcr_duplicates && !params->low_memory_mode) return CMX_ERR_INVALID;  // pairs dedup: low-memory rule only
-  cmx_ctx *ctx = new cmx_ctx;
-  // a failing CUDA call releases what has been built so far (streams, events, device buffers)
-#define CUC(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cmx_destroy(ctx); return CMX_ERR_CUDA; } } while (0)
+  std::unique_ptr<cmx_ctx> owner(new cmx_ctx);  // an early return deletes the partial context
+  cmx_ctx *ctx = owner.get();
   ctx->device = device;
   ctx->params = *params;
-  CUC(cudaSetDevice(device));
+  CU(cudaSetDevice(device));
   // The path's HBM traffic is random 16-byte table slots and short occurrence runs; CMX_L2_FETCH = 32 | 64 | 128 sets the L2
   // fetch-granularity hint for an A/B run (unset: the driver's default — the setting every committed number was measured with).
   if (const char *ev = getenv("CMX_L2_FETCH")) {
     const int gran = atoi(ev);
     if (gran == 32 || gran == 64 || gran == 128) { if (cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)gran) != cudaSuccess) cudaGetLastError(); }
   }
-  CUC(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
-  CUC(cudaStreamCreateWithFlags(&ctx->up_stream, cudaStreamNonBlocking));
-  CUC(cudaStreamCreateWithFlags(&ctx->down_stream, cudaStreamNonBlocking));
-  for (auto &e : ctx->ev) CUC(cudaEventCreate(&e));
+  CU(ctx->stream.alloc()); CU(ctx->up_stream.alloc()); CU(ctx->down_stream.alloc());
+  for (auto &e : ctx->ev) CU(e.alloc(cudaEventDefault));
   if (const char *ev = getenv("CMX_LANES")) ctx->n_lanes = std::max(1, std::min(CMX_MAX_LANES, atoi(ev)));
   for (Lane &L : ctx->lanes) {
-    CUC(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
-    for (auto &a : L.aux) CUC(cudaStreamCreateWithFlags(&a, cudaStreamNonBlocking));
-    CUC(cudaEventCreateWithFlags(&L.ev_fork, cudaEventDisableTiming));
-    for (auto &e : L.ev_join) CUC(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    for (auto &e : L.ev) CUC(cudaEventCreate(&e));
-    for (auto &e : L.ev_sub) CUC(cudaEventCreate(&e));
-    CUC(cudaEventCreateWithFlags(&L.ev_done, cudaEventDisableTiming));
-    CUC(cudaMalloc(&L.ctr, sizeof(Counters)));
-    CUC(cudaMalloc(&L.d_count, sizeof(int) * 4));
+    CU(L.stream.alloc());
+    for (auto &a : L.aux) CU(a.alloc());
+    CU(L.ev_fork.alloc(cudaEventDisableTiming));
+    for (auto &e : L.ev_join) CU(e.alloc(cudaEventDisableTiming));
+    for (Event *e : {&L.ev_tier, &L.ev_front, &L.ev_seed, &L.ev_pc, &L.ev_ver, &L.ev_pair, &L.ev_select, &L.ev_emit, &L.ev_out}) CU(e->alloc(cudaEventDefault));
+    CU(L.ctr.alloc(sizeof(Counters)));
+    CU(L.d_count.alloc(sizeof(int) * 4));
   }
   {
     std::vector<double> il(65536, 0.0);
     std::vector<int> thr(96, 0x7fffffff);
     mapq_tables_fill(il.data(), thr.data());
-    CUC(cudaMalloc(&ctx->inv_log, 65536 * sizeof(double)));
-    CUC(cudaMalloc(&ctx->pen_thr, 96 * sizeof(int)));
-    CUC(cudaMemcpy(ctx->inv_log, il.data(), 65536 * sizeof(double), cudaMemcpyHostToDevice));
-    CUC(cudaMemcpy(ctx->pen_thr, thr.data(), 96 * sizeof(int), cudaMemcpyHostToDevice));
+    CU(ctx->inv_log.alloc(65536 * sizeof(double)));
+    CU(ctx->pen_thr.alloc(96 * sizeof(int)));
+    CU(cudaMemcpy(ctx->inv_log, il.data(), 65536 * sizeof(double), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(ctx->pen_thr, thr.data(), 96 * sizeof(int), cudaMemcpyHostToDevice));
   }
   {
     std::vector<u32> mt(624);
     mt[0] = 11u;
     for (int i = 1; i < 624; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (u32)i;
-    CUC(cudaMalloc(&ctx->mt_init, 624 * sizeof(u32)));
-    CUC(cudaMemcpy(ctx->mt_init, mt.data(), 624 * sizeof(u32), cudaMemcpyHostToDevice));
+    CU(ctx->mt_init.alloc(624 * sizeof(u32)));
+    CU(cudaMemcpy(ctx->mt_init, mt.data(), 624 * sizeof(u32), cudaMemcpyHostToDevice));
   }
   // the overflow-tier kernels may use more than the default 48 KB of (static + dynamic) shared memory
-  CUC(cudaFuncSetAttribute(cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * CLUSTER_NT * 8));  // tier-0 hc = 64
-  CUC(cudaFuncSetAttribute(seed_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  CUC(cudaFuncSetAttribute(pair_candidates_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-  CUC(cudaFuncSetAttribute(verify_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  CUC(cudaFuncSetAttribute(pairing_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  CUC(cudaFuncSetAttribute(verify_split_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  CU(cudaFuncSetAttribute(cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * CLUSTER_NT * 8));  // tier-0 hc = 64
+  CU(cudaFuncSetAttribute(seed_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  CU(cudaFuncSetAttribute(pair_candidates_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+  CU(cudaFuncSetAttribute(verify_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  CU(cudaFuncSetAttribute(pairing_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  CU(cudaFuncSetAttribute(verify_split_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   const int mrl = params->max_read_length;
   if ((size_t)2 * mrl * 64 > 48 * 1024) {  // per-thread read-code columns of the verification kernels (long reads)
-    if ((size_t)2 * mrl * 64 > 200 * 1024) { cmx_destroy(ctx); return CMX_ERR_INVALID; }
-    CUC(cudaFuncSetAttribute(verify_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * mrl * 64));
+    if ((size_t)2 * mrl * 64 > 200 * 1024) return CMX_ERR_INVALID;
+    CU(cudaFuncSetAttribute(verify_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * mrl * 64));
   }
   {
     const size_t sf_smem = seed_front_smem_bytes(mrl);
-    CUC(cudaFuncSetAttribute(seed_front_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sf_smem));
-    CUC(cudaFuncSetAttribute(seed_front_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sf_smem));
+    CU(cudaFuncSetAttribute(seed_front_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sf_smem));
+    CU(cudaFuncSetAttribute(seed_front_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sf_smem));
     int per_sm = 0, n_sm = 0;
-    CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, seed_front_kernel<true>, SF_NT, sf_smem));
-    CUC(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, seed_front_kernel<true>, SF_NT, sf_smem));
+    CU(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
     ctx->sf_grid = std::max(1, per_sm) * std::max(1, n_sm);
-    int per_sm_w = 0;
-    CUC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_w, pair_candidates_cta_kernel, 32, pair_candidates_cta_smem(64, 32, mrl, 64)));
-    ctx->pcw_grid = std::max(1, per_sm_w) * std::max(1, n_sm);
   }
   for (Lane &L : ctx->lanes) {
     L.tiers[0].caps = {mrl, 64, 32, 32};
@@ -268,45 +247,14 @@ int cmx_create(cmx_ctx **out, int device, const cmx_params *params) {
     L.tiers[2].caps = {mrl * 4, 65536, 8192, 8192};
   }
   memset(&ctx->timing, 0, sizeof(ctx->timing));
-#undef CUC
-  *out = ctx;
+  *out = owner.release();
   return CMX_OK;
 }
 
 void cmx_destroy(cmx_ctx *ctx) {
   if (!ctx) return;
-  cudaSetDevice(ctx->device);
+  cudaSetDevice(ctx->device);  // (the context's owners release on its device)
   cmx_comm_destroy(ctx);
-  cudaFree(ctx->ref_seq); cudaFree(ctx->ref_off); cudaFree(ctx->ref_len);
-  cudaFree(ctx->slots); cudaFree(ctx->occ); cudaFree(ctx->inv_log); cudaFree(ctx->pen_thr); cudaFree(ctx->mt_init);
-  cudaFree(ctx->wl_slots); cudaFree(ctx->wl_pow);
-  for (DevBuf *b : {&ctx->bc_seq, &ctx->bc_qual, &ctx->seq1, &ctx->off1, &ctx->seq2, &ctx->off2, &ctx->trace}) release(*b);
-  for (Lane &L : ctx->lanes) {
-    cudaFree(L.ctr); cudaFree(L.d_count);
-    for (DevBuf *b : {&L.rescue_list, &L.verify_list, &L.emit_list, &L.nbest, &L.sel, &L.out_rec, &L.out_n, &L.offs, &L.chunk_start, &L.cub_tmp, &L.bc_key, &L.bc_ok, &L.out_compact, &L.bc_out})
-      release(*b);
-    for (auto &t : L.tiers) { release(t.mem); release(t.ovf_list); }
-    for (auto &e : L.ev) if (e) cudaEventDestroy(e);
-    for (auto &e : L.ev_sub) if (e) cudaEventDestroy(e);
-    if (L.ev_done) cudaEventDestroy(L.ev_done);
-    if (L.stream) cudaStreamDestroy(L.stream);
-    for (auto &a : L.aux) if (a) cudaStreamDestroy(a);
-    if (L.ev_fork) cudaEventDestroy(L.ev_fork);
-    for (auto &e : L.ev_join) if (e) cudaEventDestroy(e);
-  }
-  for (IngestSlot &g : ctx->ingest) {
-    for (DevBuf *b : {&g.text, &g.nl, &g.seq_start, &g.qual_start, &g.len, &g.off, &g.seq, &g.qual, &g.spans, &g.tmp, &g.stats, &g.count}) release(*b);
-    if (g.stream) cudaStreamDestroy(g.stream);
-  }
-  for (auto &e : ctx->ev) if (e) cudaEventDestroy(e);
-  for (auto &e : ctx->ev_up) cudaEventDestroy(e);
-  if (ctx->stream) cudaStreamDestroy(ctx->stream);
-  if (ctx->up_stream) cudaStreamDestroy(ctx->up_stream);
-  if (ctx->stage[0]) cudaFreeHost(ctx->stage[0]);
-  if (ctx->stage[1]) cudaFreeHost(ctx->stage[1]);
-  for (auto &e : ctx->stage_ev) if (e) cudaEventDestroy(e);
-  if (ctx->stage_stream) cudaStreamDestroy(ctx->stage_stream);
-  if (ctx->down_stream) cudaStreamDestroy(ctx->down_stream);
   delete ctx;
 }
 
@@ -321,11 +269,10 @@ static cudaError_t h2d_big(cmx_ctx *ctx, void *dst, const void *src, size_t byte
   cudaGetLastError();
   if (!plain || bytes < STAGE_BYTES / 2) return cudaMemcpy(dst, src, bytes, cudaMemcpyDefault);
   if (!ctx->stage_stream) {
-    if (cudaMallocHost(&ctx->stage[0], STAGE_BYTES) != cudaSuccess || cudaMallocHost(&ctx->stage[1], STAGE_BYTES) != cudaSuccess ||
-        cudaEventCreateWithFlags(&ctx->stage_ev[0], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ctx->stage_ev[1], cudaEventDisableTiming) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&ctx->stage_stream, cudaStreamNonBlocking) != cudaSuccess) {
+    if (ctx->stage[0].alloc(STAGE_BYTES) != cudaSuccess || ctx->stage[1].alloc(STAGE_BYTES) != cudaSuccess ||
+        ctx->stage_ev[0].alloc(cudaEventDisableTiming) != cudaSuccess || ctx->stage_ev[1].alloc(cudaEventDisableTiming) != cudaSuccess ||
+        ctx->stage_stream.alloc() != cudaSuccess) {  // (a failed alloc leaves the stream unset: the next big upload tries again)
       cudaGetLastError();
-      ctx->stage_stream = nullptr;
       return cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice);
     }
   }
@@ -339,7 +286,7 @@ static cudaError_t h2d_big(cmx_ctx *ctx, void *dst, const void *src, size_t byte
     if (rc != cudaSuccess) break;
     const int nt = 8;
     const size_t slice = ((n + nt - 1) / nt + 4095) & ~(size_t)4095;
-    char *stage = ctx->stage[b];
+    char *stage = (char *)ctx->stage[b].h;
     std::thread th[8];
     for (int t = 0; t < nt; ++t)
       th[t] = std::thread([=]() {
@@ -357,8 +304,9 @@ static cudaError_t h2d_big(cmx_ctx *ctx, void *dst, const void *src, size_t byte
 int cmx_upload_reference(cmx_ctx *ctx, uint32_t n_seq, const uint64_t *offsets, const char *concat) {
   if (!ctx || !offsets || !concat || n_seq == 0) return CMX_ERR_INVALID;
   CU(cudaSetDevice(ctx->device));
-  cudaFree(ctx->ref_seq); cudaFree(ctx->ref_off); cudaFree(ctx->ref_len);
-  ctx->ref_seq = nullptr; ctx->ref_off = nullptr; ctx->ref_len = nullptr;
+  // the old reference goes before the new one is allocated; a failed upload leaves none
+  ctx->ref_seq.reset(); ctx->ref_off.reset(); ctx->ref_len.reset();
+  ctx->n_seq = 0; ctx->h_ref_off.clear(); ctx->h_ref_len.clear();
   // device layout: [64 NUL][seq0][64.. NUL][seq1]...  every sequence start 64-byte aligned, >= 64 NULs after each
   const u64 PAD = 64;
   std::vector<u64> doff(n_seq);
@@ -370,30 +318,24 @@ int cmx_upload_reference(cmx_ctx *ctx, uint32_t n_seq, const uint64_t *offsets, 
     doff[i] = cur; dlen[i] = (u32)len;
     cur = (cur + len + PAD + 63) / 64 * 64;
   }
-  ctx->ref_bytes = cur + PAD;
-  CU(cudaMalloc(&ctx->ref_seq, ctx->ref_bytes));
-  CU(cudaMemset(ctx->ref_seq, 0, ctx->ref_bytes));
+  const u64 ref_bytes = cur + PAD;
+  DevMem<u8> seq;
+  DevMem<u64> d_off;
+  DevMem<u32> d_len;
+  CU(seq.alloc(ref_bytes));
+  CU(cudaMemset(seq, 0, ref_bytes));
   CU(cudaDeviceSynchronize());  // (the staged copies below run on their own stream)
   for (u32 i = 0; i < n_seq; ++i)
-    CU(h2d_big(ctx, ctx->ref_seq + doff[i], concat + offsets[i], dlen[i]));  // host or device source
-  CU(cudaMalloc(&ctx->ref_off, n_seq * sizeof(u64)));
-  CU(cudaMalloc(&ctx->ref_len, n_seq * sizeof(u32)));
-  CU(cudaMemcpy(ctx->ref_off, doff.data(), n_seq * sizeof(u64), cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(ctx->ref_len, dlen.data(), n_seq * sizeof(u32), cudaMemcpyHostToDevice));
+    CU(h2d_big(ctx, seq + doff[i], concat + offsets[i], dlen[i]));  // host or device source
+  CU(d_off.alloc(n_seq * sizeof(u64)));
+  CU(d_len.alloc(n_seq * sizeof(u32)));
+  CU(cudaMemcpy(d_off, doff.data(), n_seq * sizeof(u64), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(d_len, dlen.data(), n_seq * sizeof(u32), cudaMemcpyHostToDevice));
+  ctx->ref_seq = std::move(seq); ctx->ref_off = std::move(d_off); ctx->ref_len = std::move(d_len);
   ctx->n_seq = n_seq; ctx->h_ref_off = doff; ctx->h_ref_len = dlen;
   return CMX_OK;
 }
 
-// Allocate the device table for n_keys keys (load <= 0.5) and clear it.
-static int alloc_table(cmx_ctx *ctx, u64 n_keys) {
-  cudaFree(ctx->slots); ctx->slots = nullptr;
-  u64 n = 1024;
-  while (n < 2 * n_keys) n <<= 1;
-  ctx->n_slots = n;
-  CU(cudaMalloc(&ctx->slots, n * sizeof(ulonglong2)));
-  CU(cudaMemset(ctx->slots, 0xFF, n * sizeof(ulonglong2)));
-  return CMX_OK;
-}
 static int table_shift(u64 n_slots) { int lg = 0; while ((1ull << lg) < n_slots) ++lg; return 64 - lg; }
 
 // The mate-guided lookup (cta_pair_candidates.cuh) relies on every occurrence list holding distinct reference positions
@@ -402,14 +344,14 @@ __global__ void occ_check_kernel(const u64 *occ, u32 n, unsigned long long *bad)
   const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i + 1 < n && (occ[i] >> 1) == (occ[i + 1] >> 1)) atomicAdd(bad, 1ull);
 }
-static int check_occurrences(cmx_ctx *ctx) {
-  if (ctx->n_occ < 2) return CMX_OK;
-  unsigned long long *d_bad = nullptr, bad = 0;
-  CU(cudaMalloc(&d_bad, 8));
+static int check_occurrences(cmx_ctx *ctx, const u64 *occ, u32 n_occ) {
+  if (n_occ < 2) return CMX_OK;
+  DevMem<unsigned long long> d_bad;
+  unsigned long long bad = 0;
+  CU(d_bad.alloc(8));
   CU(cudaMemset(d_bad, 0, 8));
-  occ_check_kernel<<<(ctx->n_occ + 255) / 256, 256>>>(ctx->occ, ctx->n_occ, d_bad);
+  occ_check_kernel<<<(n_occ + 255) / 256, 256>>>(occ, n_occ, d_bad);
   CU(cudaMemcpy(&bad, d_bad, 8, cudaMemcpyDeviceToHost));
-  cudaFree(d_bad);
   if (bad) return fail(ctx, CMX_ERR_INVALID, "index: %llu adjacent occurrence entries share a reference position (not an index Chromap builds)", bad);
   return CMX_OK;
 }
@@ -423,35 +365,43 @@ int cmx_upload_index(cmx_ctx *ctx, int k, int w, uint32_t n_buckets, const uint3
   // the device, straight from the reference's arrays: no host-side compaction pass over a billion buckets
   const u64 nbk = n_buckets;
   const size_t nfw = (size_t)((nbk + 15) / 16);
-  u32 *d_flags = nullptr;
-  unsigned long long *d_cnt = nullptr;
-  u64 *d_k = nullptr, *d_v = nullptr;
-  CU(cudaMalloc(&d_flags, nfw * 4)); CU(cudaMalloc(&d_cnt, 8));
+  DevMem<u32> d_flags;
+  DevMem<unsigned long long> d_cnt;
+  DevMem<u64> d_k, d_v;
+  CU(d_flags.alloc(nfw * 4)); CU(d_cnt.alloc(8));
   CU(h2d_big(ctx, d_flags, flags, nfw * 4));
   CU(cudaMemset(d_cnt, 0, 8));
   khash_count_kernel<<<(unsigned)((nfw + 255) / 256), 256>>>(d_flags, nbk, d_cnt);
   unsigned long long n_keys = 0;
   CU(cudaMemcpy(&n_keys, d_cnt, 8, cudaMemcpyDeviceToHost));
-  ctx->n_keys = n_keys;
-  int rc = alloc_table(ctx, n_keys);
-  if (rc) return rc;
+  // the old index goes before the new table is allocated (a 3 Gbp table does not fit twice); a failed upload leaves none
+  ctx->slots.reset(); ctx->occ.reset();
+  ctx->n_slots = ctx->n_keys = 0; ctx->n_occ = 0; ctx->k = ctx->w = 0;
+  u64 n_slots = 1024;  // load <= 0.5
+  while (n_slots < 2 * n_keys) n_slots <<= 1;
+  DevMem<ulonglong2> slots;
+  CU(slots.alloc(n_slots * sizeof(ulonglong2)));
+  CU(cudaMemset(slots, 0xFF, n_slots * sizeof(ulonglong2)));
   const size_t CH = 1u << 25;  // buckets per chunk: 2 x 256 MB in flight
-  CU(cudaMalloc(&d_k, std::min<size_t>(nbk, CH) * 8 + 16)); CU(cudaMalloc(&d_v, std::min<size_t>(nbk, CH) * 8 + 16));
+  CU(d_k.alloc(std::min<size_t>(nbk, CH) * 8 + 16)); CU(d_v.alloc(std::min<size_t>(nbk, CH) * 8 + 16));
   for (u64 b0 = 0; b0 < nbk; b0 += CH) {
     const u64 n = std::min<u64>(CH, nbk - b0);
     CU(cudaStreamSynchronize(0));  // the previous chunk's insert kernel is done with d_k / d_v (the staged copies run on their own stream)
     CU(h2d_big(ctx, d_k, keys + b0, n * 8));
     CU(h2d_big(ctx, d_v, vals + b0, n * 8));
-    khash_insert_kernel<<<(unsigned)((n + 255) / 256), 256>>>(d_flags, d_k, d_v, b0, n, ctx->slots, ctx->n_slots - 1, table_shift(ctx->n_slots));
+    khash_insert_kernel<<<(unsigned)((n + 255) / 256), 256>>>(d_flags, d_k, d_v, b0, n, slots, n_slots - 1, table_shift(n_slots));
     CU(cudaGetLastError());
   }
   CU(cudaDeviceSynchronize());
-  cudaFree(d_flags); cudaFree(d_cnt); cudaFree(d_k); cudaFree(d_v);
-  cudaFree(ctx->occ); ctx->occ = nullptr;
-  CU(cudaMalloc(&ctx->occ, (size_t)std::max<u32>(n_occ, 1) * sizeof(u64)));
-  if (n_occ) CU(h2d_big(ctx, ctx->occ, occ, (size_t)n_occ * sizeof(u64)));
-  ctx->n_occ = n_occ; ctx->k = k; ctx->w = w;
-  return check_occurrences(ctx);
+  d_flags.reset(); d_cnt.reset(); d_k.reset(); d_v.reset();
+  DevMem<u64> d_occ;
+  CU(d_occ.alloc((size_t)std::max<u32>(n_occ, 1) * sizeof(u64)));
+  if (n_occ) CU(h2d_big(ctx, d_occ, occ, (size_t)n_occ * sizeof(u64)));
+  const int rc = check_occurrences(ctx, d_occ, n_occ);
+  if (rc) return rc;
+  ctx->slots = std::move(slots); ctx->n_slots = n_slots; ctx->occ = std::move(d_occ); ctx->n_occ = n_occ; ctx->n_keys = n_keys;
+  ctx->k = k; ctx->w = w;
+  return CMX_OK;
 }
 
 int cmx_upload_barcode_whitelist(cmx_ctx *ctx, const uint64_t *keys, const uint32_t *counts, uint64_t n, uint64_t num_sample, uint32_t bc_len,
@@ -459,27 +409,31 @@ int cmx_upload_barcode_whitelist(cmx_ctx *ctx, const uint64_t *keys, const uint3
   if (!ctx || (n && (!keys || !counts)) || bc_len == 0 || bc_len > 32) return CMX_ERR_INVALID;
   if (err_threshold < 0 || err_threshold > 1) return fail(ctx, CMX_ERR_INVALID, "--bc-error-threshold %d is not on the GPU path (0 or 1)", err_threshold);
   CU(cudaSetDevice(ctx->device));
-  cudaFree(ctx->wl_slots); ctx->wl_slots = nullptr;
+  // the old whitelist goes before the new one is allocated; a failed upload leaves none
+  ctx->wl_slots.reset(); ctx->wl_n_slots = 0; ctx->wl_active = 0;
   u64 ns = 64;
   while (ns < 2 * n) ns <<= 1;
-  CU(cudaMalloc(&ctx->wl_slots, ns * sizeof(ulonglong2)));
-  CU(cudaMemset(ctx->wl_slots, 0xFF, ns * sizeof(ulonglong2)));
+  DevMem<ulonglong2> slots;
+  CU(slots.alloc(ns * sizeof(ulonglong2)));
+  CU(cudaMemset(slots, 0xFF, ns * sizeof(ulonglong2)));
   if (n) {
-    u64 *dk; u32 *dc;
-    CU(cudaMalloc(&dk, n * 8)); CU(cudaMalloc(&dc, n * 4));
+    DevMem<u64> dk;
+    DevMem<u32> dc;
+    CU(dk.alloc(n * 8)); CU(dc.alloc(n * 4));
     CU(cudaMemcpy(dk, keys, n * 8, cudaMemcpyHostToDevice)); CU(cudaMemcpy(dc, counts, n * 4, cudaMemcpyHostToDevice));
-    wl_insert_kernel<<<(unsigned)((n + 255) / 256), 256>>>(dk, dc, n, ctx->wl_slots, ns - 1, table_shift(ns));
+    wl_insert_kernel<<<(unsigned)((n + 255) / 256), 256>>>(dk, dc, n, slots, ns - 1, table_shift(ns));
     CU(cudaGetLastError());
     CU(cudaDeviceSynchronize());
-    cudaFree(dk); cudaFree(dc);
   }
   if (!ctx->wl_pow) {
     std::vector<double> pw(41);
     for (int q = 0; q <= 40; ++q) pw[q] = pow(10.0, ((-q) / 10.0));  // host libm, chromap.cc:629-630
-    CU(cudaMalloc(&ctx->wl_pow, 41 * sizeof(double)));
-    CU(cudaMemcpy(ctx->wl_pow, pw.data(), 41 * sizeof(double), cudaMemcpyHostToDevice));
+    DevMem<double> d_pow;
+    CU(d_pow.alloc(41 * sizeof(double)));
+    CU(cudaMemcpy(d_pow, pw.data(), 41 * sizeof(double), cudaMemcpyHostToDevice));
+    ctx->wl_pow = std::move(d_pow);
   }
-  ctx->wl_n_slots = ns; ctx->wl_num_sample = num_sample; ctx->wl_bc_len = bc_len; ctx->wl_err = err_threshold; ctx->wl_prob = prob_threshold;
+  ctx->wl_slots = std::move(slots); ctx->wl_n_slots = ns; ctx->wl_num_sample = num_sample; ctx->wl_bc_len = bc_len; ctx->wl_err = err_threshold; ctx->wl_prob = prob_threshold;
   ctx->wl_output_nw = output_not_in_whitelist; ctx->wl_active = 1;
   return CMX_OK;
 }
@@ -501,12 +455,13 @@ int cmx_build_index(cmx_ctx *ctx, int k, int w) {
   CU(cudaSetDevice(ctx->device));
   IndexBuildResult r;
   std::string err;
-  const int rc = build_index_on_device(ctx->ref_seq, ctx->h_ref_off, ctx->h_ref_len, k, w, &r, &err);
+  int rc = build_index_on_device(ctx->ref_seq, ctx->h_ref_off, ctx->h_ref_len, k, w, r, err);
   if (rc != 0) return fail(ctx, rc, "%s", err.c_str());
-  cudaFree(ctx->slots); cudaFree(ctx->occ);
-  ctx->slots = r.slots; ctx->n_slots = r.n_slots; ctx->occ = r.occ; ctx->n_occ = r.n_occ; ctx->n_keys = r.n_keys;
+  rc = check_occurrences(ctx, r.occ, r.n_occ);
+  if (rc) return rc;
+  ctx->slots = std::move(r.slots); ctx->n_slots = r.n_slots; ctx->occ = std::move(r.occ); ctx->n_occ = r.n_occ; ctx->n_keys = r.n_keys;
   ctx->k = k; ctx->w = w;
-  return check_occurrences(ctx);
+  return CMX_OK;
 }
 
 // khash geometry + layout on the device: every (key, val) re-inserted with khash's own probe sequence
@@ -550,9 +505,9 @@ int cmx_download_index(cmx_ctx *ctx, uint32_t *n_buckets, uint32_t *n_keys, uint
   if (occ && ctx->n_occ) CU(cudaMemcpy(occ, ctx->occ, (size_t)ctx->n_occ * sizeof(u64), cudaMemcpyDeviceToHost));
   if (flags && keys && vals) {
     const size_t nf = nb < 16 ? 1 : nb >> 4;
-    u64 *dk = nullptr, *dv = nullptr;
-    u32 *df = nullptr;
-    CU(cudaMalloc(&dk, (size_t)nb * 8)); CU(cudaMalloc(&dv, (size_t)nb * 8)); CU(cudaMalloc(&df, nf * 4));
+    DevMem<u64> dk, dv;
+    DevMem<u32> df;
+    CU(dk.alloc((size_t)nb * 8)); CU(dv.alloc((size_t)nb * 8)); CU(df.alloc(nf * 4));
     CU(cudaMemset(dk, 0xFF, (size_t)nb * 8)); CU(cudaMemset(dv, 0, (size_t)nb * 8));
     khash_layout_kernel<<<(unsigned)((ctx->n_slots + 255) / 256), 256>>>(ctx->slots, ctx->n_slots, dk, dv, nb - 1);
     khash_flags_kernel<<<(unsigned)((nf + 255) / 256), 256>>>(dk, dv, nb, df);
@@ -561,7 +516,6 @@ int cmx_download_index(cmx_ctx *ctx, uint32_t *n_buckets, uint32_t *n_keys, uint
     CU(cudaMemcpy(keys, dk, (size_t)nb * 8, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(vals, dv, (size_t)nb * 8, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(flags, df, nf * 4, cudaMemcpyDeviceToHost));
-    cudaFree(dk); cudaFree(dv); cudaFree(df);
   }
   return CMX_OK;
 }
@@ -572,7 +526,7 @@ static cudaError_t tier_prepare(Tier &t, int n_slots, const int *pair_list, bool
   if (n_slots > t.slots_cap) {
     const size_t want_slots = (size_t)n_slots + n_slots / 8 + 16;
     const size_t bytes = scratch_layout(t.caps, want_slots, interleaved, o);
-    release(t.mem);
+    t.mem.reset();
     cudaError_t e = ensure(t.mem, bytes);
     if (e != cudaSuccess) return e;
     t.slots_cap = (int)want_slots;
@@ -629,7 +583,7 @@ static int upload_batch(cmx_ctx *ctx, const cmx_batch *in, DevBatch *B) {
 }
 
 struct BatchAcc {  // per-call accumulators over sub-batches
-  float ms_seed = 0, ms_pc = 0, ms_ver = 0, ms_pair = 0, ms_minimizer = 0, ms_probe = 0, ms_cluster = 0, ms_select = 0, ms_emit = 0;
+  float ms_seed = 0, ms_pc = 0, ms_ver = 0, ms_pair = 0, ms_minimizer = 0, ms_cluster = 0, ms_select = 0, ms_emit = 0;
   u64 launches = 0, n_overflow = 0;
   Counters c;
   u64 tier_pairs[N_TIERS] = {0, 0, 0};
@@ -637,21 +591,10 @@ struct BatchAcc {  // per-call accumulators over sub-batches
   BatchAcc() { memset(&c, 0, sizeof(c)); }
 };
 
-#define CUL(call)                                                                                  \
-  do {                                                                                             \
-    cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess) {                                                                       \
-      char b_[512];                                                                                \
-      snprintf(b_, sizeof(b_), "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); \
-      L.err = b_;                                                                                  \
-      return CMX_ERR_CUDA;                                                                         \
-    }                                                                                              \
-  } while (0)
-
 struct LaneJob {  // what one lane maps in one call: pairs [p0, p0 + n) of the call's batch
   u32 p0 = 0, n = 0;
   u32 piece = 0, piece0 = 0;                       // reads arrive in pieces of `piece` pairs; this lane's first piece index
-  const std::vector<cudaEvent_t> *piece_ready = nullptr;
+  const std::vector<Event> *piece_ready = nullptr;
   const u8 *bc_seq = nullptr, *bc_qual = nullptr;  // device, already offset to p0
   u32 bc_len = 0;
   cudaEvent_t bc_ready = nullptr;
@@ -665,7 +608,8 @@ struct LaneJob {  // what one lane maps in one call: pairs [p0, p0 + n) of the c
 // The whole device pipeline over pairs already resident in HBM (or landing piece by piece); records compacted in
 // read order into the lane's buffer.  Synchronous on the lane's stream; safe to run one lane per host thread.
 static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
-  CUL(cudaSetDevice(ctx->device));
+  std::string &err = L.err;  // where CUE reports: lanes run on their own host threads and must not write ctx->err
+  CUE(cudaSetDevice(ctx->device));
   const u32 n = J.n;
   BatchAcc &acc = J.acc;
   DevBatch B = Bfull;  // view of this lane's pairs: pair index i of the lane = pair p0 + i of the call
@@ -680,26 +624,26 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
   R.seq = ctx->ref_seq; R.off = ctx->ref_off; R.len = ctx->ref_len; R.n_seq = ctx->n_seq;
   MapqTables T;
   T.inv_log = ctx->inv_log; T.pen_thr = ctx->pen_thr;
-  CUL(ensure(L.nbest, (size_t)n * 4)); CUL(ensure(L.sel, (size_t)n * mb * 4));
+  CUE(ensure(L.nbest, (size_t)n * 4)); CUE(ensure(L.sel, (size_t)n * mb * 4));
   const bool sam = ctx->params.output_format == 4;
   const size_t rec_bytes = sam ? sizeof(OutSam) : sizeof(OutRecord);
-  CUL(ensure(L.out_rec, (size_t)n * mb * rec_bytes)); CUL(ensure(L.out_n, (size_t)(n + 1) * 4));
-  CUL(ensure(L.offs, (size_t)(n + 1) * 8));
+  CUE(ensure(L.out_rec, (size_t)n * mb * rec_bytes)); CUE(ensure(L.out_n, (size_t)(n + 1) * 4));
+  CUE(ensure(L.offs, (size_t)(n + 1) * 8));
   OutRecord *dst = J.dst;
-  if (!dst) { CUL(ensure(L.out_compact, (size_t)n * mb * rec_bytes)); dst = (OutRecord *)L.out_compact.p; }
+  if (!dst) { CUE(ensure(L.out_compact, (size_t)n * mb * rec_bytes)); dst = (OutRecord *)L.out_compact.p; }
   J.dst = dst;
   u64 *bc_dst = nullptr;
-  if (J.want_bc && J.bc_seq) { CUL(ensure(L.bc_out, (size_t)n * mb * 8)); bc_dst = (u64 *)L.bc_out.p; }
-  CUL(cudaMemsetAsync(L.nbest.p, 0, (size_t)n * 4, st));
-  CUL(cudaMemsetAsync(L.out_n.p, 0, (size_t)(n + 1) * 4, st));
-  CUL(cudaMemsetAsync(L.ctr, 0, sizeof(Counters), st));
+  if (J.want_bc && J.bc_seq) { CUE(ensure(L.bc_out, (size_t)n * mb * 8)); bc_dst = (u64 *)L.bc_out.p; }
+  CUE(cudaMemsetAsync(L.nbest.p, 0, (size_t)n * 4, st));
+  CUE(cudaMemsetAsync(L.out_n.p, 0, (size_t)(n + 1) * 4, st));
+  CUE(cudaMemsetAsync(L.ctr, 0, sizeof(Counters), st));
   if (J.bc_seq) {  // the barcode gate, when barcodes came with the batch
     DevWhitelist W;
     W.slots = ctx->wl_slots; W.mask = ctx->wl_n_slots ? ctx->wl_n_slots - 1 : 0; W.shift = ctx->wl_n_slots ? table_shift(ctx->wl_n_slots) : 0;
     W.num_sample = (double)ctx->wl_num_sample; W.pow_tab = ctx->wl_pow; W.err_threshold = ctx->wl_err; W.prob_threshold = ctx->wl_prob;
     W.output_not_in_whitelist = ctx->wl_output_nw; W.active = ctx->wl_active;
-    CUL(ensure(L.bc_key, (size_t)n * 8)); CUL(ensure(L.bc_ok, (size_t)n));
-    if (J.bc_ready) CUL(cudaStreamWaitEvent(st, J.bc_ready, 0));
+    CUE(ensure(L.bc_key, (size_t)n * 8)); CUE(ensure(L.bc_ok, (size_t)n));
+    if (J.bc_ready) CUE(cudaStreamWaitEvent(st, J.bc_ready, 0));
     barcode_kernel<<<(n + 127) / 128, 128, 0, st>>>(W, J.bc_seq, J.bc_qual, (int)J.bc_len, (int)n, (u64 *)L.bc_key.p, (u8 *)L.bc_ok.p, L.ctr);
     acc.launches += 1;
     B.bc_ok = (const u8 *)L.bc_ok.p;
@@ -711,11 +655,11 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
   const int TB = 128;
   for (int t = 0; t < N_TIERS && n_slots > 0; ++t) {
     Tier &tier = L.tiers[t];
-    CUL(tier_prepare(tier, n_slots, pair_list, t == 0));
+    CUE(tier_prepare(tier, n_slots, pair_list, t == 0));
     const Scratch S = tier.view;
-    cudaEvent_t e0 = L.ev[5], e1 = L.ev[6], e2 = L.ev[7], e3 = L.ev[8], e4 = L.ev[9];
+    cudaEvent_t e0 = L.ev_tier, e1 = L.ev_seed, e2 = L.ev_pc, e3 = L.ev_ver, e4 = L.ev_pair;
     int cluster_passes = 1;
-    CUL(cudaEventRecord(e0, st));
+    CUE(cudaEventRecord(e0, st));
     if (t == 0) {
       // front end: [adapter trimming] + length filter + minimizers + index probe in one kernel over staged read tiles
       // (seed_front.cuh).  When the reads arrive in pieces on the upload stream, one grid per piece starts as soon as
@@ -724,7 +668,7 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
       const u32 piece = J.piece_ready ? J.piece : n;
       for (u32 q = 0, p0 = 0; p0 < n; ++q, p0 += piece) {
         const u32 np = std::min(piece, n - p0);
-        if (J.piece_ready) CUL(cudaStreamWaitEvent(st, (*J.piece_ready)[J.piece0 + q], 0));
+        if (J.piece_ready) CUE(cudaStreamWaitEvent(st, (*J.piece_ready)[J.piece0 + q], 0));
         if (P.trim) {
           Scratch V = S;
           V.n_slots = (int)np; V.rmeta += 2 * (size_t)p0; V.pmeta += p0;
@@ -746,10 +690,9 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
       prep_kernel<<<(n_slots + TB - 1) / TB, TB, 0, st>>>(P, B, S);
     }
     if (t == 0) {
-      CUL(ensure(L.rescue_list, (size_t)n_slots * 4)); CUL(ensure(L.verify_list, (size_t)n_slots * 8));  // verify_list: cluster's, then verify's
-      CUL(cudaMemsetAsync(L.d_count + 1, 0, 3 * sizeof(int), st));
-      CUL(cudaEventRecord(L.ev_sub[0], st));
-      CUL(cudaEventRecord(L.ev_sub[1], st));
+      CUE(ensure(L.rescue_list, (size_t)n_slots * 4)); CUE(ensure(L.verify_list, (size_t)n_slots * 8));  // verify_list: cluster's, then verify's
+      CUE(cudaMemsetAsync(L.d_count + 1, 0, 3 * sizeof(int), st));
+      CUE(cudaEventRecord(L.ev_front, st));
       {
         // first-pass tile: enough rows for a typical read (about 2L/(w+1) minimizers, most of them single hits)
         int rows0 = (2 * ctx->params.max_read_length / (ctx->w + 1) + 15) / 16 * 16;  // 16 rows at 2x50, 48 at 2x150
@@ -759,25 +702,25 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
         if (rows0 < S.caps.hc)
           cluster_kernel<<<(2 * n_slots + CLUSTER_NT - 1) / CLUSTER_NT, CLUSTER_NT, (size_t)S.caps.hc * CLUSTER_NT * 8, st>>>(P, ix, S, L.ctr, 1, S.caps.hc, (int *)L.verify_list.p, L.d_count + 3);
       }
-      CUL(cudaEventRecord(e1, st));
+      CUE(cudaEventRecord(e1, st));
 
       pair_candidates_kernel<<<(n_slots + TB - 1) / TB, TB, 0, st>>>(P, ix, S, L.ctr, 0, (int *)L.rescue_list.p, L.d_count + 1);
       pair_candidates_kernel<<<(n_slots + 63) / 64, 64, 0, st>>>(P, ix, S, L.ctr, 1, (int *)L.rescue_list.p, L.d_count + 1);
-      CUL(cudaEventRecord(e2, st));
+      CUE(cudaEventRecord(e2, st));
       if (P.split) verify_split_kernel<<<(2 * n_slots + TB - 1) / TB, TB, 0, st>>>(P, R, B, S, L.ctr);
       else {
         verify_kernel<<<(2 * n_slots + TB - 1) / TB, TB, 0, st>>>(P, R, B, S, L.ctr, 0, (int *)L.verify_list.p, L.d_count + 2);
         verify_kernel<<<(2 * n_slots + 63) / 64, 64, (size_t)2 * S.caps.maxmm * 64, st>>>(P, R, B, S, L.ctr, 1, (int *)L.verify_list.p, L.d_count + 2);
       }
-      CUL(cudaEventRecord(e3, st));
+      CUE(cudaEventRecord(e3, st));
       if (P.split) pairing_split_kernel<<<(n_slots + TB - 1) / TB, TB, 0, st>>>(P, S, (int *)L.nbest.p);
       else pairing_kernel<<<(n_slots + TB - 1) / TB, TB, 0, st>>>(P, S, (int *)L.nbest.p);
-      CUL(cudaEventRecord(e4, st));
+      CUE(cudaEventRecord(e4, st));
     } else {  // overflow tiers: one CTA per read / pair; shared-memory sort buffers sized to the tier
       auto cap_of = [](int n) { int c = 1; while (c < n) c <<= 1; return std::min(c, CTA_SORT_SMEM_MAX); };
       const int c_seed = cap_of(2 * tier.caps.hc), c_pc = cap_of(tier.caps.hc), c_ver = cap_of(tier.caps.cc), c_pair = cap_of(tier.caps.mc);
       seed_cta_kernel<<<2 * n_slots, CTA_NT, (size_t)c_seed * 11 + (size_t)(tier.caps.maxmm + 1) * 12 + 16, st>>>(P, ix, B, S, L.tiers[0].view, L.ctr, c_seed);
-      CUL(cudaEventRecord(e1, st));
+      CUE(cudaEventRecord(e1, st));
       {
         const int lcap = std::min(tier.caps.cc, 512), fcap = 2 * tier.caps.cc;
         // the last tier's shared-memory lists leave room for two CTAs per SM only: sixteen warps each instead of four keep as
@@ -786,29 +729,29 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
         const int pc_nt = pc_smem > 64 * 1024 ? PC_CTA_NT_MAX : CTA_NT;
         pair_candidates_cta_kernel<<<n_slots, pc_nt, pc_smem, st>>>(P, ix, S, L.ctr, c_pc, lcap, fcap, nullptr, nullptr);
       }
-      CUL(cudaEventRecord(e2, st));
+      CUE(cudaEventRecord(e2, st));
       if (P.split) verify_split_cta_kernel<<<2 * n_slots, CTA_NT, (size_t)c_ver * 9, st>>>(P, R, B, S, L.ctr, c_ver);
       else verify_cta_kernel<<<2 * n_slots, tier.caps.cc > 1024 ? VERIFY_NT_MAX : CTA_NT, (size_t)c_ver * 9 + 2 * (size_t)tier.caps.maxmm + 16, st>>>(P, R, B, S, L.ctr, c_ver);
-      CUL(cudaEventRecord(e3, st));
+      CUE(cudaEventRecord(e3, st));
       if (P.split) pairing_split_kernel<<<(n_slots + TB - 1) / TB, TB, 0, st>>>(P, S, (int *)L.nbest.p);
       else pairing_cta_kernel<<<n_slots, CTA_NT, (size_t)c_pair * 10, st>>>(P, S, (int *)L.nbest.p, c_pair);
-      CUL(cudaEventRecord(e4, st));
+      CUE(cudaEventRecord(e4, st));
     }
     // kernels launched above: tier 0 = front end (counted per piece) + cluster (1 or 2 passes) + pair_candidates x2 +
     // verify (x2 unless split) + pairing; overflow tiers = prep + four CTA kernels
     if (t == 0) acc.launches += cluster_passes + 2 + (P.split ? 1 : 2) + 1;
     else acc.launches += 5;
-    CUL(ensure(tier.ovf_list, (size_t)n_slots * 4));
-    CUL(cudaMemsetAsync(L.d_count, 0, sizeof(int), st));
+    CUE(ensure(tier.ovf_list, (size_t)n_slots * 4));
+    CUE(cudaMemsetAsync(L.d_count, 0, sizeof(int), st));
     collect_overflow_kernel<<<(n_slots + 255) / 256, 256, 0, st>>>(S, (int *)tier.ovf_list.p, L.d_count);
     acc.launches += 1;
     int n_ovf = 0;
-    CUL(cudaMemcpyAsync(&n_ovf, L.d_count, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUL(cudaStreamSynchronize(st));
-    CUL(cudaGetLastError());
+    CUE(cudaMemcpyAsync(&n_ovf, L.d_count, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUE(cudaStreamSynchronize(st));
+    CUE(cudaGetLastError());
     float f;
     cudaEventElapsedTime(&f, e0, e1); acc.ms_seed += f;
-    if (t == 0) { cudaEventElapsedTime(&f, e0, L.ev_sub[0]); acc.ms_minimizer += f; cudaEventElapsedTime(&f, L.ev_sub[0], L.ev_sub[1]); acc.ms_probe += f; cudaEventElapsedTime(&f, L.ev_sub[1], e1); acc.ms_cluster += f; }
+    if (t == 0) { cudaEventElapsedTime(&f, e0, L.ev_front); acc.ms_minimizer += f; cudaEventElapsedTime(&f, L.ev_front, e1); acc.ms_cluster += f; }
     cudaEventElapsedTime(&f, e1, e2); acc.ms_pc += f;
     cudaEventElapsedTime(&f, e2, e3); acc.ms_ver += f;
     cudaEventElapsedTime(&f, e3, e4); acc.ms_pair += f;
@@ -816,11 +759,11 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
     if (n_ovf > 0 && t + 1 < N_TIERS) {
       // deterministic order for the next tier: sort the pair list (atomic append order is arbitrary)
       std::vector<int> h(n_ovf);
-      CUL(cudaMemcpyAsync(h.data(), tier.ovf_list.p, (size_t)n_ovf * 4, cudaMemcpyDeviceToHost, st));
-      CUL(cudaStreamSynchronize(st));
+      CUE(cudaMemcpyAsync(h.data(), tier.ovf_list.p, (size_t)n_ovf * 4, cudaMemcpyDeviceToHost, st));
+      CUE(cudaStreamSynchronize(st));
       std::sort(h.begin(), h.end());
-      CUL(cudaMemcpyAsync(tier.ovf_list.p, h.data(), (size_t)n_ovf * 4, cudaMemcpyHostToDevice, st));
-      CUL(cudaStreamSynchronize(st));
+      CUE(cudaMemcpyAsync(tier.ovf_list.p, h.data(), (size_t)n_ovf * 4, cudaMemcpyHostToDevice, st));
+      CUE(cudaStreamSynchronize(st));
       pair_list = (const int *)tier.ovf_list.p;
     } else if (n_ovf > 0) {
       n_overflow_final = n_ovf;
@@ -832,39 +775,39 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
   for (u32 b0 = 0; b0 < n; b0 += (u32)ctx->params.batch_size) taskloop_chunks(b0, std::min<u32>((u32)ctx->params.batch_size, n - b0), chunks);
   const int n_chunks = (int)chunks.size();
   chunks.push_back((int)n);
-  CUL(ensure(L.chunk_start, chunks.size() * 4));
-  CUL(cudaEventRecord(L.ev[2], st));
-  CUL(cudaMemcpyAsync(L.chunk_start.p, chunks.data(), chunks.size() * 4, cudaMemcpyHostToDevice, st));
+  CUE(ensure(L.chunk_start, chunks.size() * 4));
+  CUE(cudaEventRecord(L.ev_select, st));
+  CUE(cudaMemcpyAsync(L.chunk_start.p, chunks.data(), chunks.size() * 4, cudaMemcpyHostToDevice, st));
   select_kernel<<<(n_chunks + 3) / 4, 128, 0, st>>>(P, n_chunks, (const int *)L.chunk_start.p, (const int *)L.nbest.p, (int *)L.sel.p, ctx->mt_init);
-  CUL(cudaEventRecord(L.ev[3], st));
+  CUE(cudaEventRecord(L.ev_emit, st));
   // the overflow tiers' emits (few pairs, long per-thread sweeps) run beside tier 0's on their own streams
-  if (tiers_used > 1) CUL(cudaEventRecord(L.ev_fork, st));
+  if (tiers_used > 1) CUE(cudaEventRecord(L.ev_fork, st));
   for (int t = tiers_used - 1; t >= 0; --t) {
     const Scratch S = L.tiers[t].view;
     cudaStream_t es = t == 0 ? st : L.aux[t - 1];
-    if (t > 0) CUL(cudaStreamWaitEvent(es, L.ev_fork, 0));
+    if (t > 0) CUE(cudaStreamWaitEvent(es, L.ev_fork, 0));
     if (P.split) emit_split_kernel<<<(S.n_slots + TB - 1) / TB, TB, 0, es>>>(P, R, B, T, S, (const int *)L.sel.p, (OutPairs *)L.out_rec.p, (int *)L.out_n.p, L.ctr);
     else if (sam && P.se) emit_sam_se_kernel<<<(S.n_slots + TB - 1) / TB, TB, 0, es>>>(P, R, B, T, S, (const int *)L.sel.p, (OutSam *)L.out_rec.p, (int *)L.out_n.p, L.ctr);
     else if (sam) emit_sam_kernel<<<(S.n_slots + TB - 1) / TB, TB, 0, es>>>(P, R, B, T, S, (const int *)L.sel.p, (OutSam *)L.out_rec.p, (int *)L.out_n.p, L.ctr);
     else if (P.se) emit_se_kernel<<<(S.n_slots + TB - 1) / TB, TB, 0, es>>>(P, R, B, T, S, (const int *)L.sel.p, (OutRecord *)L.out_rec.p, (int *)L.out_n.p, L.ctr);
     else if (t > 0) emit_cta_kernel<<<S.n_slots, CTA_NT, 0, es>>>(P, R, B, T, S, (const int *)L.sel.p, (OutRecord *)L.out_rec.p, (int *)L.out_n.p, L.ctr);
     else {
-      CUL(ensure(L.emit_list, (size_t)S.n_slots * mb * sizeof(int4)));
-      CUL(cudaMemsetAsync(L.d_count + 2, 0, sizeof(int), es));  // (verify's list counter: free by now)
+      CUE(ensure(L.emit_list, (size_t)S.n_slots * mb * sizeof(int4)));
+      CUE(cudaMemsetAsync(L.d_count + 2, 0, sizeof(int), es));  // (verify's list counter: free by now)
       emit_kernel<<<(S.n_slots + TB - 1) / TB, TB, 0, es>>>(P, R, B, T, S, (const int *)L.sel.p, (OutRecord *)L.out_rec.p, (int *)L.out_n.p, L.ctr, (int4 *)L.emit_list.p,
                                                            L.d_count + 2);
       // the pairs whose start coordinates need the bit-vector traceback (indels); the grid covers the worst case, idle threads leave at once
       emit_dp_kernel<<<(unsigned)(((size_t)S.n_slots * mb + TB - 1) / TB), TB, 0, es>>>(P, R, B, T, S, (OutRecord *)L.out_rec.p, (const int4 *)L.emit_list.p, L.d_count + 2);
       acc.launches += 1;
     }
-    if (t > 0) CUL(cudaEventRecord(L.ev_join[t - 1], es));
+    if (t > 0) CUE(cudaEventRecord(L.ev_join[t - 1], es));
   }
-  for (int t = 1; t < tiers_used; ++t) CUL(cudaStreamWaitEvent(st, L.ev_join[t - 1], 0));
+  for (int t = 1; t < tiers_used; ++t) CUE(cudaStreamWaitEvent(st, L.ev_join[t - 1], 0));
   acc.launches += 1 + tiers_used;
   // read-order compaction
   size_t tmp_bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (const int *)L.out_n.p, (u64 *)L.offs.p, (int)n + 1, st);
-  CUL(ensure(L.cub_tmp, tmp_bytes));
+  CUE(ensure(L.cub_tmp, tmp_bytes));
   // out_n has n entries plus one trailing zero so that offs[n] = total
   cub::DeviceScan::ExclusiveSum(L.cub_tmp.p, tmp_bytes, (const int *)L.out_n.p, (u64 *)L.offs.p, (int)n + 1, st);
   if (sam) compact_words_kernel<<<(n + 255) / 256, 256, 0, st>>>((int)n, mb, (int)(rec_bytes / 4), (const u32 *)L.out_rec.p, (const int *)L.out_n.p, (const u64 *)L.offs.p, (u32 *)dst);
@@ -875,15 +818,15 @@ static int run_lane(cmx_ctx *ctx, Lane &L, const DevBatch &Bfull, LaneJob &J) {
     acc.launches += 1;
   }
   u64 total = 0;
-  CUL(cudaEventRecord(L.ev[4], st));
-  CUL(cudaMemcpyAsync(&total, (u64 *)L.offs.p + n, 8, cudaMemcpyDeviceToHost, st));
+  CUE(cudaEventRecord(L.ev_out, st));
+  CUE(cudaMemcpyAsync(&total, (u64 *)L.offs.p + n, 8, cudaMemcpyDeviceToHost, st));
   Counters hc;
-  CUL(cudaMemcpyAsync(&hc, L.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, st));
-  CUL(cudaStreamSynchronize(st));
-  CUL(cudaGetLastError());
+  CUE(cudaMemcpyAsync(&hc, L.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, st));
+  CUE(cudaStreamSynchronize(st));
+  CUE(cudaGetLastError());
   float f;
-  cudaEventElapsedTime(&f, L.ev[2], L.ev[3]); acc.ms_select += f;
-  cudaEventElapsedTime(&f, L.ev[3], L.ev[4]); acc.ms_emit += f;
+  cudaEventElapsedTime(&f, L.ev_select, L.ev_emit); acc.ms_select += f;
+  cudaEventElapsedTime(&f, L.ev_emit, L.ev_out); acc.ms_emit += f;
   {
     u64 *a = (u64 *)&acc.c;
     const u64 *b = (const u64 *)&hc;
@@ -934,14 +877,14 @@ int cmx_map_batch_pe(cmx_ctx *ctx, const cmx_batch *in, cmx_records *out, void *
     CU(ensure(ctx->seq1, b1 + 64)); CU(ensure(ctx->seq2, b2 + 64));
     CU(ensure(ctx->off1, (size_t)(n + 1) * 4)); CU(ensure(ctx->off2, (size_t)(n + 1) * 4));
     n_pieces = (n + ps - 1) / ps;
-    while (ctx->ev_up.size() < n_pieces) { cudaEvent_t e; CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->ev_up.push_back(e); }
+    while (ctx->ev_up.size() < n_pieces) { Event e; CU(e.alloc(cudaEventDisableTiming)); ctx->ev_up.push_back(std::move(e)); }
     CU(cudaMemcpyAsync(ctx->off1.p, in->off1, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, up));
     if (!se) CU(cudaMemcpyAsync(ctx->off2.p, in->off2, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, up));
     if (bc) {
       CU(ensure(ctx->bc_seq, (size_t)n * in->bc_len + 16)); CU(ensure(ctx->bc_qual, (size_t)n * in->bc_len + 16));
       CU(cudaMemcpyAsync(ctx->bc_seq.p, in->bc_seq, (size_t)n * in->bc_len, cudaMemcpyHostToDevice, up));
       CU(cudaMemcpyAsync(ctx->bc_qual.p, in->bc_qual, (size_t)n * in->bc_len, cudaMemcpyHostToDevice, up));
-      if (!ctx->ev_bc) CU(cudaEventCreateWithFlags(&ctx->ev_bc, cudaEventDisableTiming));
+      if (!ctx->ev_bc) CU(ctx->ev_bc.alloc(cudaEventDisableTiming));
       CU(cudaEventRecord(ctx->ev_bc, up));
       bcs = (const u8 *)ctx->bc_seq.p; bcq = (const u8 *)ctx->bc_qual.p;
     }
@@ -964,7 +907,7 @@ int cmx_map_batch_pe(cmx_ctx *ctx, const cmx_batch *in, cmx_records *out, void *
     LaneJob &J = jobs[l];
     J.p0 = s0 * bs; J.n = std::min(n, s1 * bs) - J.p0;
     if (pieces) { J.piece = ps; J.piece0 = s0 * (bs / ps); J.piece_ready = &ctx->ev_up; }
-    if (bc) { J.bc_seq = bcs + (size_t)J.p0 * in->bc_len; J.bc_qual = bcq + (size_t)J.p0 * in->bc_len; J.bc_len = in->bc_len; J.bc_ready = pieces ? ctx->ev_bc : nullptr; }
+    if (bc) { J.bc_seq = bcs + (size_t)J.p0 * in->bc_len; J.bc_qual = bcq + (size_t)J.p0 * in->bc_len; J.bc_len = in->bc_len; J.bc_ready = pieces ? ctx->ev_bc.h : nullptr; }
     J.want_bc = bc && out->barcode_keys;
     if (out->on_device && n_lanes == 1) J.dst = (OutRecord *)out->records;
   }
@@ -1015,7 +958,7 @@ int cmx_map_batch_pe(cmx_ctx *ctx, const cmx_batch *in, cmx_records *out, void *
   for (int l = 0; l < n_lanes; ++l) {
     const BatchAcc &a = jobs[l].acc;
     acc.ms_seed += a.ms_seed; acc.ms_pc += a.ms_pc; acc.ms_ver += a.ms_ver; acc.ms_pair += a.ms_pair; acc.ms_minimizer += a.ms_minimizer;
-    acc.ms_probe += a.ms_probe; acc.ms_cluster += a.ms_cluster; acc.ms_select += a.ms_select; acc.ms_emit += a.ms_emit;
+    acc.ms_cluster += a.ms_cluster; acc.ms_select += a.ms_select; acc.ms_emit += a.ms_emit;
     acc.launches += a.launches; acc.n_overflow += a.n_overflow;
     u64 *x = (u64 *)&acc.c;
     const u64 *y = (const u64 *)&a.c;
@@ -1030,7 +973,7 @@ int cmx_map_batch_pe(cmx_ctx *ctx, const cmx_batch *in, cmx_records *out, void *
   memset(&tm, 0, sizeof(tm));
   // stage times are sums over the lanes' own streams; lanes overlap, so they add up to more than total_ms
   tm.h2d_ms = ms_h2d; tm.d2h_ms = 0;  // record copies run on the lanes' own streams, overlapped with other lanes' kernels
-  tm.seed_ms = acc.ms_seed; tm.front_ms = acc.ms_minimizer + acc.ms_probe; tm.reserved_ms = 0; tm.cluster_ms = acc.ms_cluster;
+  tm.seed_ms = acc.ms_seed; tm.front_ms = acc.ms_minimizer; tm.reserved_ms = 0; tm.cluster_ms = acc.ms_cluster;
   tm.pair_candidates_ms = acc.ms_pc; tm.verify_ms = acc.ms_ver; tm.pairing_ms = acc.ms_pair; tm.select_ms = acc.ms_select; tm.emit_ms = acc.ms_emit;
   tm.total_ms = ms_call;
   tm.n_minimizers = acc.c.n_minimizers; tm.n_probe_steps = acc.c.n_probe_steps; tm.n_found = acc.c.n_found; tm.n_occ_reads = acc.c.n_occ_reads;
@@ -1064,7 +1007,7 @@ int cmx_ingest_fastq(cmx_ctx *ctx, int slot, const char *text, uint64_t n_bytes,
   if (text[n_bytes - 1] != '\n') return fail(ctx, CMX_ERR_INVALID, "cmx_ingest_fastq: the chunk must end at a record boundary (cmx_fastq_cut)");
   CU(cudaSetDevice(ctx->device));
   IngestSlot &g = ctx->ingest[slot];
-  if (!g.stream) CU(cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking));
+  if (!g.stream) CU(g.stream.alloc());
   cudaStream_t st = g.stream;
   const u32 nb = (u32)n_bytes;
   CU(ensure(g.text, n_bytes + 16)); CU(ensure(g.nl, ((size_t)nb + 16) * 4)); CU(ensure(g.count, 16)); CU(ensure(g.stats, sizeof(IngestStats)));
@@ -1128,7 +1071,7 @@ int cmx_set_lanes(cmx_ctx *ctx, int n_lanes) {
     CU(cudaSetDevice(ctx->device));
     CU(cudaDeviceSynchronize());
     for (Lane &L : ctx->lanes)
-      for (Tier &t : L.tiers) { release(t.mem); release(t.ovf_list); t.slots_cap = 0; }
+      for (Tier &t : L.tiers) { t.mem.reset(); t.ovf_list.reset(); t.slots_cap = 0; }
   }
   ctx->n_lanes = n_lanes;
   return CMX_OK;
@@ -1202,15 +1145,16 @@ int cmx_stage_minimizers(cmx_ctx *ctx, const cmx_batch *in, uint64_t *out_hash, 
   int rc = upload_batch(ctx, in, &B);
   if (rc) return rc;
   const size_t R = 2 * (size_t)in->n_pairs;
-  u64 *dh; u32 *dp; int *dn;
-  CU(cudaMalloc(&dh, R * stride * 8)); CU(cudaMalloc(&dp, R * stride * 4)); CU(cudaMalloc(&dn, R * 4));
+  DevMem<u64> dh;
+  DevMem<u32> dp;
+  DevMem<int> dn;
+  CU(dh.alloc(R * stride * 8)); CU(dp.alloc(R * stride * 4)); CU(dn.alloc(R * 4));
   stage_minimizers_kernel<<<(unsigned)((R + 127) / 128), 128, 0, ctx->stream>>>(B, ctx->k, ctx->w, dh, dp, dn, stride);
   CU(cudaStreamSynchronize(ctx->stream));
   CU(cudaGetLastError());
   CU(cudaMemcpy(out_hash, dh, R * stride * 8, cudaMemcpyDeviceToHost));
   CU(cudaMemcpy(out_pos, dp, R * stride * 4, cudaMemcpyDeviceToHost));
   CU(cudaMemcpy(out_n, dn, R * 4, cudaMemcpyDeviceToHost));
-  cudaFree(dh); cudaFree(dp); cudaFree(dn);
   return CMX_OK;
 }
 
@@ -1231,14 +1175,14 @@ int cmx_stage_probe(cmx_ctx *ctx, const uint64_t *hashes, uint64_t n, uint8_t *f
   CU(cudaSetDevice(ctx->device));
   DevIndex ix;
   ix.slots = ctx->slots; ix.n_slots_mask = ctx->n_slots - 1; ix.shift = table_shift(ctx->n_slots); ix.occ = ctx->occ; ix.n_occ = ctx->n_occ; ix.k = ctx->k; ix.w = ctx->w;
-  u64 *dh, *dk, *dv; u8 *df;
-  CU(cudaMalloc(&dh, n * 8 + 8)); CU(cudaMalloc(&dk, n * 8 + 8)); CU(cudaMalloc(&dv, n * 8 + 8)); CU(cudaMalloc(&df, n + 8));
+  DevMem<u64> dh, dk, dv;
+  DevMem<u8> df;
+  CU(dh.alloc(n * 8 + 8)); CU(dk.alloc(n * 8 + 8)); CU(dv.alloc(n * 8 + 8)); CU(df.alloc(n + 8));
   CU(cudaMemcpy(dh, hashes, n * 8, cudaMemcpyHostToDevice));
   if (n) stage_probe_kernel<<<(unsigned)((n + 255) / 256), 256>>>(ix, dh, n, df, dk, dv);
   CU(cudaDeviceSynchronize());
   CU(cudaGetLastError());
   CU(cudaMemcpy(found, df, n, cudaMemcpyDeviceToHost)); CU(cudaMemcpy(key, dk, n * 8, cudaMemcpyDeviceToHost)); CU(cudaMemcpy(val, dv, n * 8, cudaMemcpyDeviceToHost));
-  cudaFree(dh); cudaFree(dk); cudaFree(dv); cudaFree(df);
   return CMX_OK;
 }
 
@@ -1254,15 +1198,15 @@ __global__ void stage_align_kernel(int e, int L, const u8 *pat, const u8 *txt, u
 int cmx_stage_banded_align(cmx_ctx *ctx, int e, int read_len, const char *patterns, const char *texts, uint64_t n, int32_t *num_errors, int32_t *end_pos) {
   if (!ctx || !patterns || !texts || !num_errors || !end_pos || e < 1 || e > 15 || read_len < 1) return CMX_ERR_INVALID;
   CU(cudaSetDevice(ctx->device));
-  u8 *dp, *dt; int *de, *dq;
+  DevMem<u8> dp, dt;
+  DevMem<int> de, dq;
   const size_t pb = n * (size_t)(read_len + 2 * e), tb = n * (size_t)read_len;
-  CU(cudaMalloc(&dp, pb + 8)); CU(cudaMalloc(&dt, tb + 8)); CU(cudaMalloc(&de, n * 4 + 8)); CU(cudaMalloc(&dq, n * 4 + 8));
+  CU(dp.alloc(pb + 8)); CU(dt.alloc(tb + 8)); CU(de.alloc(n * 4 + 8)); CU(dq.alloc(n * 4 + 8));
   CU(cudaMemcpy(dp, patterns, pb, cudaMemcpyHostToDevice)); CU(cudaMemcpy(dt, texts, tb, cudaMemcpyHostToDevice));
   if (n) stage_align_kernel<<<(unsigned)((n + 127) / 128), 128>>>(e, read_len, dp, dt, n, de, dq);
   CU(cudaDeviceSynchronize());
   CU(cudaGetLastError());
   CU(cudaMemcpy(num_errors, de, n * 4, cudaMemcpyDeviceToHost)); CU(cudaMemcpy(end_pos, dq, n * 4, cudaMemcpyDeviceToHost));
-  cudaFree(dp); cudaFree(dt); cudaFree(de); cudaFree(dq);
   return CMX_OK;
 }
 
@@ -1282,8 +1226,9 @@ int cmx_stage_cta_sort(cmx_ctx *ctx, uint64_t *keys, uint8_t *tags, uint32_t n, 
   CU(cudaSetDevice(ctx->device));
   size_t cap = 1;
   while (cap < n) cap <<= 1;
-  u64 *dk; u8 *dt;
-  CU(cudaMalloc(&dk, cap * 8 + 8)); CU(cudaMalloc(&dt, cap + 8));
+  DevMem<u64> dk;
+  DevMem<u8> dt;
+  CU(dk.alloc(cap * 8 + 8)); CU(dt.alloc(cap + 8));
   CU(cudaMemcpy(dk, keys, (size_t)n * 8, cudaMemcpyHostToDevice));
   if (tags) CU(cudaMemcpy(dt, tags, n, cudaMemcpyHostToDevice));
   stage_cta_sort_kernel<<<1, CTA_NT, (size_t)sm_cap * 9>>>(dk, dt, (int)n, (int)sm_cap, tags ? 1 : 0);
@@ -1291,7 +1236,6 @@ int cmx_stage_cta_sort(cmx_ctx *ctx, uint64_t *keys, uint8_t *tags, uint32_t n, 
   CU(cudaGetLastError());
   CU(cudaMemcpy(keys, dk, (size_t)n * 8, cudaMemcpyDeviceToHost));
   if (tags) CU(cudaMemcpy(tags, dt, n, cudaMemcpyDeviceToHost));
-  cudaFree(dk); cudaFree(dt);
   return CMX_OK;
 }
 
@@ -1465,14 +1409,12 @@ static int pp_device(cmx_ctx *ctx, const PpParams &P, PpRecord *d_a, u64 *d_bca,
   if (n > 0x7FFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "post-processing: more than 2^31-1 records in one call");
   const bool bc = P.kind == PP_BED_BC;
   cudaStream_t st = ctx->stream;
-  u64 *d_k0 = nullptr, *d_k1 = nullptr, *d_nsel = nullptr;
-  u32 *d_i0 = nullptr, *d_i1 = nullptr;
-  u8 *d_head = nullptr, *d_keep = nullptr;
-  void *d_tmp = nullptr;
-  auto cleanup = [&]() { cudaFree(d_k0); cudaFree(d_k1); cudaFree(d_nsel); cudaFree(d_i0); cudaFree(d_i1); cudaFree(d_head); cudaFree(d_keep); cudaFree(d_tmp); };
-#define PPCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cleanup(); return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } } while (0)
-  PPCU(cudaMalloc(&d_k0, n * 8)); PPCU(cudaMalloc(&d_k1, n * 8)); PPCU(cudaMalloc(&d_i0, n * 4)); PPCU(cudaMalloc(&d_i1, n * 4));
-  PPCU(cudaMalloc(&d_head, n)); PPCU(cudaMalloc(&d_keep, n)); PPCU(cudaMalloc(&d_nsel, 16));
+  DevMem<u64> d_k0, d_k1, d_nsel;
+  DevMem<u32> d_i0, d_i1;
+  DevMem<u8> d_head, d_keep;
+  DevMem<> d_tmp;
+  CU(d_k0.alloc(n * 8)); CU(d_k1.alloc(n * 8)); CU(d_i0.alloc(n * 4)); CU(d_i1.alloc(n * 4));
+  CU(d_head.alloc(n)); CU(d_keep.alloc(n)); CU(d_nsel.alloc(16));
   const unsigned nb = (unsigned)((n + 255) / 256);
   if (!P.low_mem && P.tn5 && P.kind != PP_PAIRS) pp_tn5_kernel<<<nb, 256, 0, st>>>(P.kind, P.se, d_a, n);  // chromap.h:1322-1355: before the sort
   pp_iota_kernel<<<nb, 256, 0, st>>>(d_i0, n);
@@ -1480,18 +1422,18 @@ static int pp_device(cmx_ctx *ctx, const PpParams &P, PpRecord *d_a, u64 *d_bca,
   cub::DoubleBuffer<u32> di(d_i0, d_i1);
   size_t tmp_bytes = 0, need = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, dk, di, (int)n, 0, 64, st);
-  cub::DeviceSelect::Flagged(nullptr, need, d_a, d_keep, d_b, d_nsel, (int)n, st);
+  cub::DeviceSelect::Flagged(nullptr, need, d_a, d_keep.p, d_b, d_nsel.p, (int)n, st);
   tmp_bytes = std::max(tmp_bytes, need);
-  cub::DeviceSelect::Flagged(nullptr, need, d_bca, d_keep, d_bcb, d_nsel, (int)n, st);
+  cub::DeviceSelect::Flagged(nullptr, need, d_bca, d_keep.p, d_bcb, d_nsel.p, (int)n, st);
   tmp_bytes = std::max(tmp_bytes, need);
-  PPCU(cudaMalloc(&d_tmp, tmp_bytes));
+  CU(d_tmp.alloc(tmp_bytes));
   // only the bits a key word can hold are sorted: word 0 (rid | start, or rid1 | rid2) up to its largest value in this call;
   // pp_key_word bounds the others: the 32-bit alignment lengths; length alone; mapq | direction | unique | read id
   u64 max0 = 0;
-  PPCU(cudaMemsetAsync(d_nsel, 0, 16, st));
+  CU(cudaMemsetAsync(d_nsel, 0, 16, st));
   pp_max_key0_kernel<<<std::min(nb, 1184u), 256, 0, st>>>(P.kind, d_a, n, d_nsel);
-  PPCU(cudaMemcpyAsync(&max0, d_nsel, 8, cudaMemcpyDeviceToHost, st));
-  PPCU(cudaStreamSynchronize(st));
+  CU(cudaMemcpyAsync(&max0, d_nsel, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   int bits0 = 1;
   while (bits0 < 64 && (max0 >> bits0)) ++bits0;
   for (int w = pp_n_words(P.kind) - 1; w >= 0; --w) {  // least significant word first; every pass is stable
@@ -1501,19 +1443,17 @@ static int pp_device(cmx_ctx *ctx, const PpParams &P, PpRecord *d_a, u64 *d_bca,
     else if (P.kind == PP_PAIRS) bits = w == 2 ? 40 : 64;
     else if (bc) bits = w == 1 ? 16 : (w == 3 ? 56 : 64);
     else if (w == 2) bits = 32;
-    PPCU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dk, di, (int)n, 0, bits, st));
+    CU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dk, di, (int)n, 0, bits, st));
   }
   pp_gather_kernel<<<nb, 256, 0, st>>>(d_a, bc ? d_bca : nullptr, di.Current(), n, d_b, d_bcb);
   pp_head_kernel<<<nb, 256, 0, st>>>(P.kind, P.se, P.dedup, d_b, bc ? d_bcb : nullptr, n, d_head);
   pp_resolve_kernel<<<nb, 256, 0, st>>>(P, d_b, bc ? d_bcb : nullptr, d_head, n, d_a, bc ? d_bca : nullptr, d_keep);
-  PPCU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_a, d_keep, d_b, d_nsel, (int)n, st));
-  if (bc) PPCU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_bca, d_keep, d_bcb, d_nsel + 1, (int)n, st));
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_a, d_keep.p, d_b, d_nsel.p, (int)n, st));
+  if (bc) CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_bca, d_keep.p, d_bcb, d_nsel + 1, (int)n, st));
   u64 nsel = 0;
-  PPCU(cudaMemcpyAsync(&nsel, d_nsel, 8, cudaMemcpyDeviceToHost, st));
-  PPCU(cudaStreamSynchronize(st));
-  PPCU(cudaGetLastError());
-#undef PPCU
-  cleanup();
+  CU(cudaMemcpyAsync(&nsel, d_nsel, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
   *nsel_out = nsel;
   return CMX_OK;
 }
@@ -1534,22 +1474,18 @@ int cmx_postprocess_gpu(cmx_ctx *ctx, void *records, uint64_t *barcode_keys, uin
   if (P.kind == PP_PAIRS && barcode_keys) return fail(ctx, CMX_ERR_INVALID, "barcodes are not supported with pairs output");
   const bool bc = P.kind == PP_BED_BC;
   cudaStream_t st = ctx->stream;
-  PpRecord *d_a = nullptr, *d_b = nullptr;
-  u64 *d_bca = nullptr, *d_bcb = nullptr;
-  auto cleanup = [&]() { cudaFree(d_a); cudaFree(d_b); cudaFree(d_bca); cudaFree(d_bcb); };
-#define PPCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cleanup(); return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } } while (0)
-  PPCU(cudaMalloc(&d_a, n * sizeof(PpRecord))); PPCU(cudaMalloc(&d_b, n * sizeof(PpRecord)));
-  if (bc) { PPCU(cudaMalloc(&d_bca, n * 8)); PPCU(cudaMalloc(&d_bcb, n * 8)); }
-  PPCU(cudaMemcpyAsync(d_a, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
-  if (bc) PPCU(cudaMemcpyAsync(d_bca, barcode_keys, n * 8, cudaMemcpyHostToDevice, st));
+  DevMem<PpRecord> d_a, d_b;
+  DevMem<u64> d_bca, d_bcb;
+  CU(d_a.alloc(n * sizeof(PpRecord))); CU(d_b.alloc(n * sizeof(PpRecord)));
+  if (bc) { CU(d_bca.alloc(n * 8)); CU(d_bcb.alloc(n * 8)); }
+  CU(cudaMemcpyAsync(d_a, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
+  if (bc) CU(cudaMemcpyAsync(d_bca, barcode_keys, n * 8, cudaMemcpyHostToDevice, st));
   u64 nsel = 0;
   const int rc = pp_device(ctx, P, d_a, d_bca, n, d_b, d_bcb, &nsel);
-  if (rc != CMX_OK) { cleanup(); return rc; }
-  if (nsel) PPCU(cudaMemcpyAsync(records, d_b, nsel * sizeof(PpRecord), cudaMemcpyDeviceToHost, st));
-  if (bc && nsel) PPCU(cudaMemcpyAsync(barcode_keys, d_bcb, nsel * 8, cudaMemcpyDeviceToHost, st));
-  PPCU(cudaStreamSynchronize(st));
-#undef PPCU
-  cleanup();
+  if (rc != CMX_OK) return rc;
+  if (nsel) CU(cudaMemcpyAsync(records, d_b, nsel * sizeof(PpRecord), cudaMemcpyDeviceToHost, st));
+  if (bc && nsel) CU(cudaMemcpyAsync(barcode_keys, d_bcb, nsel * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   *n_out = nsel;
   return CMX_OK;
 }
@@ -1600,6 +1536,14 @@ NcclApi &nccl_api() {
 const int NCCL_UINT8 = 1, NCCL_UINT64 = 5;  // ncclDataType_t
 }  // namespace
 
+#define NC(call)                                                                                                      \
+  do {                                                                                                                \
+    const int r_ = (call);                                                                                            \
+    if (r_ != 0)                                                                                                      \
+      return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call,                                       \
+                  nccl_api().GetErrorString ? nccl_api().GetErrorString(r_) : "NCCL error");                          \
+  } while (0)
+
 int cmx_comm_unique_id(void *id128) {
   if (!id128) return CMX_ERR_INVALID;
   NcclApi &N = nccl_api();
@@ -1648,92 +1592,88 @@ int cmx_dedup_exchange(cmx_ctx *ctx, const void *records, const uint64_t *barcod
   cudaStream_t st = ctx->stream;
   const bool bc = barcode_keys != nullptr;
   const int tw = bc ? 3 : 2, R = ctx->comm_size, rank = ctx->comm_rank;
-  PpRecord *d_rec = nullptr, *d_out = nullptr;
-  u64 *d_bc = nullptr, *d_outbc = nullptr, *d_cnt = nullptr, *d_send = nullptr, *d_all = nullptr, *d_k0 = nullptr, *d_k1 = nullptr, *d_nsel = nullptr;
-  u32 *d_i0 = nullptr, *d_i1 = nullptr, *d_sel = nullptr, *d_selc = nullptr;
-  u8 *d_head = nullptr, *d_keep = nullptr, *d_dups = nullptr, *d_dupsc = nullptr;
-  void *d_tmp = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  auto cleanup = [&]() {
-    if (!on_device) { cudaFree(d_rec); cudaFree(d_bc); cudaFree(d_out); cudaFree(d_outbc); }
-    cudaFree(d_cnt); cudaFree(d_send); cudaFree(d_all); cudaFree(d_k0); cudaFree(d_k1); cudaFree(d_nsel); cudaFree(d_i0); cudaFree(d_i1);
-    cudaFree(d_sel); cudaFree(d_selc); cudaFree(d_head); cudaFree(d_keep); cudaFree(d_dups); cudaFree(d_dupsc); cudaFree(d_tmp);
-    for (auto &e : ev) if (e) cudaEventDestroy(e);
-  };
-#define XCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cleanup(); return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } } while (0)
-#define XNC(call) do { int r_ = (call); if (r_ != 0) { cleanup(); return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, N.GetErrorString ? N.GetErrorString(r_) : "NCCL error"); } } while (0)
-  for (auto &e : ev) XCU(cudaEventCreate(&e));
+  PpRecord *d_rec = nullptr, *d_out = nullptr;  // the caller's device buffers, or copies of its host records
+  u64 *d_bc = nullptr, *d_outbc = nullptr;
+  DevMem<PpRecord> rec_copy, out_copy;
+  DevMem<u64> bc_copy, outbc_copy, d_cnt, d_send, d_all, d_k0, d_k1, d_nsel;
+  DevMem<u32> d_i0, d_i1, d_sel, d_selc;
+  DevMem<u8> d_head, d_keep, d_dups, d_dupsc;
+  DevMem<> d_tmp;
+  Event ev[4];
+  for (auto &e : ev) CU(e.alloc(cudaEventDefault));
   if (on_device) { d_rec = (PpRecord *)records; d_bc = (u64 *)barcode_keys; d_out = (PpRecord *)out_records; d_outbc = (u64 *)out_barcode_keys; }
   else {
-    XCU(cudaMalloc(&d_rec, std::max<u64>(n, 1) * sizeof(PpRecord))); XCU(cudaMalloc(&d_out, std::max<u64>(n, 1) * sizeof(PpRecord)));
-    XCU(cudaMemcpyAsync(d_rec, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
-    if (bc) { XCU(cudaMalloc(&d_bc, std::max<u64>(n, 1) * 8)); XCU(cudaMalloc(&d_outbc, std::max<u64>(n, 1) * 8)); XCU(cudaMemcpyAsync(d_bc, barcode_keys, n * 8, cudaMemcpyHostToDevice, st)); }
+    CU(rec_copy.alloc(std::max<u64>(n, 1) * sizeof(PpRecord))); CU(out_copy.alloc(std::max<u64>(n, 1) * sizeof(PpRecord)));
+    d_rec = rec_copy; d_out = out_copy;
+    CU(cudaMemcpyAsync(d_rec, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
+    if (bc) {
+      CU(bc_copy.alloc(std::max<u64>(n, 1) * 8)); CU(outbc_copy.alloc(std::max<u64>(n, 1) * 8));
+      d_bc = bc_copy; d_outbc = outbc_copy;
+      CU(cudaMemcpyAsync(d_bc, barcode_keys, n * 8, cudaMemcpyHostToDevice, st));
+    }
   }
   // sizes: an 8-byte all-gather of the record counts
-  XCU(cudaMalloc(&d_cnt, (size_t)(R + 1) * 8));
-  XCU(cudaMemcpyAsync(d_cnt + R, &n, 8, cudaMemcpyHostToDevice, st));
-  XNC(N.AllGather(d_cnt + R, d_cnt, 1, NCCL_UINT64, ctx->nccl_comm, st));
+  CU(d_cnt.alloc((size_t)(R + 1) * 8));
+  CU(cudaMemcpyAsync(d_cnt + R, &n, 8, cudaMemcpyHostToDevice, st));
+  NC(N.AllGather(d_cnt + R, d_cnt, 1, NCCL_UINT64, ctx->nccl_comm, st));
   std::vector<u64> cnt(R);
-  XCU(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)R * 8, cudaMemcpyDeviceToHost, st));
-  XCU(cudaStreamSynchronize(st));
+  CU(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)R * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   u64 n_pad = 1, n_total = 0;
   for (u64 c : cnt) { n_pad = std::max(n_pad, c); n_total += c; }
   const u64 n_all = n_pad * (u64)R;
-  if (n_all >= 0xFFFFFFFFull) { cleanup(); return fail(ctx, CMX_ERR_INVALID, "cmx_dedup_exchange: %llu gathered tuples exceed 2^32", (unsigned long long)n_all); }
+  if (n_all >= 0xFFFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "cmx_dedup_exchange: %llu gathered tuples exceed 2^32", (unsigned long long)n_all);
   // pack -> ONE all-gather of the tuples -> sort -> decide
-  XCU(cudaMalloc(&d_send, n_pad * tw * 8)); XCU(cudaMalloc(&d_all, n_all * tw * 8));
-  XCU(cudaMalloc(&d_k0, n_all * 8)); XCU(cudaMalloc(&d_k1, n_all * 8)); XCU(cudaMalloc(&d_i0, n_all * 4)); XCU(cudaMalloc(&d_i1, n_all * 4));
-  XCU(cudaMalloc(&d_head, n_all)); XCU(cudaMalloc(&d_keep, n_all)); XCU(cudaMalloc(&d_dups, n_all)); XCU(cudaMalloc(&d_dupsc, std::max<u64>(n, 1)));
-  XCU(cudaMalloc(&d_sel, n_all * 4)); XCU(cudaMalloc(&d_selc, std::max<u64>(n, 1) * 4)); XCU(cudaMalloc(&d_nsel, 16));
-  XCU(cudaEventRecord(ev[0], st));
+  CU(d_send.alloc(n_pad * tw * 8)); CU(d_all.alloc(n_all * tw * 8));
+  CU(d_k0.alloc(n_all * 8)); CU(d_k1.alloc(n_all * 8)); CU(d_i0.alloc(n_all * 4)); CU(d_i1.alloc(n_all * 4));
+  CU(d_head.alloc(n_all)); CU(d_keep.alloc(n_all)); CU(d_dups.alloc(n_all)); CU(d_dupsc.alloc(std::max<u64>(n, 1)));
+  CU(d_sel.alloc(n_all * 4)); CU(d_selc.alloc(std::max<u64>(n, 1) * 4)); CU(d_nsel.alloc(16));
+  CU(cudaEventRecord(ev[0], st));
   ex_pack_kernel<<<(unsigned)((n_pad + 255) / 256), 256, 0, st>>>(d_rec, d_bc, n, n_pad, bc ? 1 : 0, d_send);
-  XCU(cudaEventRecord(ev[1], st));
-  XNC(N.AllGather(d_send, d_all, n_pad * tw * 8, NCCL_UINT8, ctx->nccl_comm, st));
-  XCU(cudaEventRecord(ev[2], st));
+  CU(cudaEventRecord(ev[1], st));
+  NC(N.AllGather(d_send, d_all, n_pad * tw * 8, NCCL_UINT8, ctx->nccl_comm, st));
+  CU(cudaEventRecord(ev[2], st));
   const unsigned nb = (unsigned)((n_all + 255) / 256);
   pp_iota_kernel<<<nb, 256, 0, st>>>(d_i0, n_all);
   cub::DoubleBuffer<u64> dk(d_k0, d_k1);
   cub::DoubleBuffer<u32> di(d_i0, d_i1);
   size_t tmp_bytes = 0, need = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, dk, di, (int)n_all, 0, 64, st);
-  cub::DeviceSelect::Flagged(nullptr, need, d_sel, d_keep, d_selc, d_nsel, (int)n_all, st);
+  cub::DeviceSelect::Flagged(nullptr, need, d_sel.p, d_keep.p, d_selc.p, d_nsel.p, (int)n_all, st);
   tmp_bytes = std::max(tmp_bytes, need);
-  XCU(cudaMalloc(&d_tmp, tmp_bytes));
+  CU(d_tmp.alloc(tmp_bytes));
   // least significant key first, every pass stable: bulk (b, a); barcoded (low 48 bits of b, barcode, length, a)
   const int passes_bulk[2] = {4, 3}, passes_bc[4] = {0, 1, 2, 3};
   for (int q = 0; q < (bc ? 4 : 2); ++q) {
     const int pass = bc ? passes_bc[q] : passes_bulk[q];
     ex_key_kernel<<<nb, 256, 0, st>>>(d_all, tw, pass, di.Current(), n_all, dk.Current());
-    XCU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dk, di, (int)n_all, 0, pass == 2 ? 16 : 64, st));
+    CU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dk, di, (int)n_all, 0, pass == 2 ? 16 : 64, st));
   }
   // padding sorts last (a = ~0): only the first n_total sorted entries are records
   if (n_total) {
     const unsigned nbt = (unsigned)((n_total + 255) / 256);
     ex_head_kernel<<<nbt, 256, 0, st>>>(d_all, tw, p.remove_pcr_duplicates, di.Current(), n_total, d_head);
     ex_resolve_kernel<<<nbt, 256, 0, st>>>(d_all, tw, di.Current(), d_head, n_total, n_pad, rank, p.mapq_threshold, d_keep, d_sel, d_dups);
-    XCU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_sel, d_keep, d_selc, d_nsel, (int)n_total, st));
-    XCU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_dups, d_keep, d_dupsc, d_nsel + 1, (int)n_total, st));
-  } else XCU(cudaMemsetAsync(d_nsel, 0, 16, st));
+    CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_sel.p, d_keep.p, d_selc.p, d_nsel.p, (int)n_total, st));
+    CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_dups.p, d_keep.p, d_dupsc.p, d_nsel + 1, (int)n_total, st));
+  } else CU(cudaMemsetAsync(d_nsel, 0, 16, st));
   u64 nsel = 0;
-  XCU(cudaMemcpyAsync(&nsel, d_nsel, 8, cudaMemcpyDeviceToHost, st));
-  XCU(cudaStreamSynchronize(st));
+  CU(cudaMemcpyAsync(&nsel, d_nsel, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   if (nsel) ex_gather_kernel<<<(unsigned)((nsel + 255) / 256), 256, 0, st>>>(d_rec, d_bc, d_selc, d_dupsc, p.remove_pcr_duplicates, nsel, d_out, bc ? d_outbc : nullptr);
-  XCU(cudaEventRecord(ev[3], st));
+  CU(cudaEventRecord(ev[3], st));
   if (!on_device && nsel) {
-    XCU(cudaMemcpyAsync(out_records, d_out, nsel * sizeof(PpRecord), cudaMemcpyDeviceToHost, st));
-    if (bc && out_barcode_keys) XCU(cudaMemcpyAsync(out_barcode_keys, d_outbc, nsel * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out_records, d_out, nsel * sizeof(PpRecord), cudaMemcpyDeviceToHost, st));
+    if (bc && out_barcode_keys) CU(cudaMemcpyAsync(out_barcode_keys, d_outbc, nsel * 8, cudaMemcpyDeviceToHost, st));
   }
-  XCU(cudaStreamSynchronize(st));
-  XCU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
   if (stats) {
     cudaEventElapsedTime(&stats->pack_ms, ev[0], ev[1]);
     cudaEventElapsedTime(&stats->allgather_ms, ev[1], ev[2]);
     cudaEventElapsedTime(&stats->resolve_ms, ev[2], ev[3]);
     stats->bytes_sent = n_pad * tw * 8; stats->bytes_received = n_all * tw * 8; stats->n_global = n_total; stats->n_ranks = (uint32_t)R;
   }
-#undef XCU
-#undef XNC
-  cleanup();
   *n_out = nsel;
   return CMX_OK;
 }
@@ -1757,35 +1697,28 @@ int cmx_dedup_shuffle(cmx_ctx *ctx, const void *records, const uint64_t *barcode
   cudaStream_t st = ctx->stream;
   const bool bc = barcode_keys != nullptr;
   const int R = ctx->comm_size, rank = ctx->comm_rank;
-  PpRecord *d_rec = nullptr, *d_send = nullptr, *d_recv = nullptr, *d_res = nullptr;
-  u64 *d_bc = nullptr, *d_sendbc = nullptr, *d_recvbc = nullptr, *d_resbc = nullptr, *d_a = nullptr, *d_samp = nullptr, *d_all0 = nullptr, *d_all1 = nullptr,
-      *d_split = nullptr, *d_off = nullptr, *d_offall = nullptr;
-  u32 *d_d0 = nullptr, *d_d1 = nullptr, *d_i0 = nullptr, *d_i1 = nullptr;
-  void *d_tmp = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  auto cleanup = [&]() {
-    if (!on_device) { cudaFree(d_rec); cudaFree(d_bc); }
-    cudaFree(d_send); cudaFree(d_recv); cudaFree(d_res); cudaFree(d_sendbc); cudaFree(d_recvbc); cudaFree(d_resbc); cudaFree(d_a); cudaFree(d_samp);
-    cudaFree(d_all0); cudaFree(d_all1); cudaFree(d_split); cudaFree(d_off); cudaFree(d_offall); cudaFree(d_d0); cudaFree(d_d1); cudaFree(d_i0); cudaFree(d_i1);
-    cudaFree(d_tmp);
-    for (auto &e : ev) if (e) cudaEventDestroy(e);
-  };
-#define XCU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cleanup(); return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } } while (0)
-#define XNC(call) do { int r_ = (call); if (r_ != 0) { cleanup(); return fail(ctx, CMX_ERR_CUDA, "%s:%d %s: %s", __FILE__, __LINE__, #call, N.GetErrorString ? N.GetErrorString(r_) : "NCCL error"); } } while (0)
-  for (auto &e : ev) XCU(cudaEventCreate(&e));
+  PpRecord *d_rec = nullptr;  // the caller's device records, or a copy of its host records
+  u64 *d_bc = nullptr;
+  DevMem<PpRecord> rec_copy, d_send, d_recv, d_res;
+  DevMem<u64> bc_copy, d_sendbc, d_recvbc, d_resbc, d_a, d_samp, d_all0, d_all1, d_split, d_off, d_offall;
+  DevMem<u32> d_d0, d_d1, d_i0, d_i1;
+  DevMem<> d_tmp;
+  Event ev[4];
+  for (auto &e : ev) CU(e.alloc(cudaEventDefault));
   const u64 n1 = std::max<u64>(n, 1);
   if (on_device) { d_rec = (PpRecord *)records; d_bc = (u64 *)barcode_keys; }
   else {
-    XCU(cudaMalloc(&d_rec, n1 * sizeof(PpRecord)));
-    XCU(cudaMemcpyAsync(d_rec, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
-    if (bc) { XCU(cudaMalloc(&d_bc, n1 * 8)); XCU(cudaMemcpyAsync(d_bc, barcode_keys, n * 8, cudaMemcpyHostToDevice, st)); }
+    CU(rec_copy.alloc(n1 * sizeof(PpRecord)));
+    d_rec = rec_copy;
+    CU(cudaMemcpyAsync(d_rec, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
+    if (bc) { CU(bc_copy.alloc(n1 * 8)); d_bc = bc_copy; CU(cudaMemcpyAsync(d_bc, barcode_keys, n * 8, cudaMemcpyHostToDevice, st)); }
   }
   const u64 n_samp = (u64)R * SH_SAMPLE;
-  XCU(cudaMalloc(&d_a, n1 * 8)); XCU(cudaMalloc(&d_samp, SH_SAMPLE * 8)); XCU(cudaMalloc(&d_all0, n_samp * 8)); XCU(cudaMalloc(&d_all1, n_samp * 8));
-  XCU(cudaMalloc(&d_split, (size_t)std::max(R - 1, 1) * 8)); XCU(cudaMalloc(&d_off, (size_t)(R + 1) * 8)); XCU(cudaMalloc(&d_offall, (size_t)R * (R + 1) * 8));
-  XCU(cudaMalloc(&d_d0, n1 * 4)); XCU(cudaMalloc(&d_d1, n1 * 4)); XCU(cudaMalloc(&d_i0, n1 * 4)); XCU(cudaMalloc(&d_i1, n1 * 4));
-  XCU(cudaMalloc(&d_send, n1 * sizeof(PpRecord)));
-  if (bc) XCU(cudaMalloc(&d_sendbc, n1 * 8));
+  CU(d_a.alloc(n1 * 8)); CU(d_samp.alloc(SH_SAMPLE * 8)); CU(d_all0.alloc(n_samp * 8)); CU(d_all1.alloc(n_samp * 8));
+  CU(d_split.alloc((size_t)std::max(R - 1, 1) * 8)); CU(d_off.alloc((size_t)(R + 1) * 8)); CU(d_offall.alloc((size_t)R * (R + 1) * 8));
+  CU(d_d0.alloc(n1 * 4)); CU(d_d1.alloc(n1 * 4)); CU(d_i0.alloc(n1 * 4)); CU(d_i1.alloc(n1 * 4));
+  CU(d_send.alloc(n1 * sizeof(PpRecord)));
+  if (bc) CU(d_sendbc.alloc(n1 * 8));
   size_t tmp_bytes = 0, need = 0;
   {
     cub::DoubleBuffer<u64> ks(d_all0, d_all1);
@@ -1794,83 +1727,83 @@ int cmx_dedup_shuffle(cmx_ctx *ctx, const void *records, const uint64_t *barcode
     cub::DeviceRadixSort::SortPairs(nullptr, need, dd, di, (int)n1, 0, 32, st);
     tmp_bytes = std::max(tmp_bytes, need);
   }
-  XCU(cudaMalloc(&d_tmp, tmp_bytes));
+  CU(d_tmp.alloc(tmp_bytes));
   // ---- partition: splitters from an all-gathered sample, destination of every record, records grouped by destination
-  XCU(cudaEventRecord(ev[0], st));
+  CU(cudaEventRecord(ev[0], st));
   const unsigned nb = (unsigned)((n1 + 255) / 256);
   if (n) sh_key_kernel<<<nb, 256, 0, st>>>(d_rec, n, d_a);
   sh_sample_kernel<<<(SH_SAMPLE + 255) / 256, 256, 0, st>>>(d_a, n, d_samp);
-  XNC(N.AllGather(d_samp, d_all0, SH_SAMPLE, NCCL_UINT64, ctx->nccl_comm, st));
+  NC(N.AllGather(d_samp, d_all0, SH_SAMPLE, NCCL_UINT64, ctx->nccl_comm, st));
   cub::DoubleBuffer<u64> ks(d_all0, d_all1);
-  XCU(cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, ks, (int)n_samp, 0, 64, st));
+  CU(cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, ks, (int)n_samp, 0, 64, st));
   std::vector<u64> samp(n_samp), split(std::max(R - 1, 1), 0);
-  XCU(cudaMemcpyAsync(samp.data(), ks.Current(), n_samp * 8, cudaMemcpyDeviceToHost, st));
-  XCU(cudaStreamSynchronize(st));
+  CU(cudaMemcpyAsync(samp.data(), ks.Current(), n_samp * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   const u64 valid = (u64)(std::lower_bound(samp.begin(), samp.end(), (u64)EX_PAD) - samp.begin());  // padding sorts last
   for (int j = 1; j < R; ++j) split[j - 1] = valid ? samp[valid * (u64)j / (u64)R] : 0ull;           // the same on every rank
-  XCU(cudaMemcpyAsync(d_split, split.data(), split.size() * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_split, split.data(), split.size() * 8, cudaMemcpyHostToDevice, st));
   int dest_bits = 1;
   while ((1 << dest_bits) < R) ++dest_bits;
   cub::DoubleBuffer<u32> dd(d_d0, d_d1), di(d_i0, d_i1);
   if (n) {
     sh_dest_kernel<<<nb, 256, 0, st>>>(d_a, n, d_split, R - 1, dd.Current());
     pp_iota_kernel<<<nb, 256, 0, st>>>(di.Current(), n);
-    XCU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dd, di, (int)n, 0, dest_bits, st));  // stable: mapping order kept inside a destination
+    CU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dd, di, (int)n, 0, dest_bits, st));  // stable: mapping order kept inside a destination
     pp_gather_kernel<<<nb, 256, 0, st>>>(d_rec, bc ? d_bc : nullptr, di.Current(), n, d_send, d_sendbc);
   }
   sh_bounds_kernel<<<(R + 1 + 63) / 64, 64, 0, st>>>(dd.Current(), n, R, d_off);
-  XNC(N.AllGather(d_off, d_offall, (size_t)(R + 1), NCCL_UINT64, ctx->nccl_comm, st));
+  NC(N.AllGather(d_off, d_offall, (size_t)(R + 1), NCCL_UINT64, ctx->nccl_comm, st));
   std::vector<u64> offall((size_t)R * (R + 1));
-  XCU(cudaMemcpyAsync(offall.data(), d_offall, offall.size() * 8, cudaMemcpyDeviceToHost, st));
-  XCU(cudaStreamSynchronize(st));
+  CU(cudaMemcpyAsync(offall.data(), d_offall, offall.size() * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
   auto cnt = [&](int from, int to) { return offall[(size_t)from * (R + 1) + to + 1] - offall[(size_t)from * (R + 1) + to]; };
   u64 n_recv = 0, n_global = 0;
   std::vector<u64> roff(R + 1, 0);
   for (int q = 0; q < R; ++q) { roff[q] = n_recv; n_recv += cnt(q, rank); n_global += offall[(size_t)q * (R + 1) + R]; }
   roff[R] = n_recv;
-  if (n_recv >= 0x7FFFFFFFull) { cleanup(); return fail(ctx, CMX_ERR_INVALID, "cmx_dedup_shuffle: %llu records in this rank's key range exceed 2^31-1", (unsigned long long)n_recv); }
+  if (n_recv >= 0x7FFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "cmx_dedup_shuffle: %llu records in this rank's key range exceed 2^31-1", (unsigned long long)n_recv);
   const u64 nr1 = std::max<u64>(n_recv, 1);
-  XCU(cudaMalloc(&d_recv, nr1 * sizeof(PpRecord))); XCU(cudaMalloc(&d_res, nr1 * sizeof(PpRecord)));
-  if (bc) { XCU(cudaMalloc(&d_recvbc, nr1 * 8)); XCU(cudaMalloc(&d_resbc, nr1 * 8)); }
+  CU(d_recv.alloc(nr1 * sizeof(PpRecord))); CU(d_res.alloc(nr1 * sizeof(PpRecord)));
+  if (bc) { CU(d_recvbc.alloc(nr1 * 8)); CU(d_resbc.alloc(nr1 * 8)); }
   // ---- shuffle: every record travels once, to the rank that owns its key range
-  XCU(cudaEventRecord(ev[1], st));
-  XNC(N.GroupStart());
+  CU(cudaEventRecord(ev[1], st));
+  NC(N.GroupStart());
   for (int q = 0; q < R; ++q) {
     const u64 so = offall[(size_t)rank * (R + 1) + q], sc = cnt(rank, q), rc = cnt(q, rank);
     if (q == rank) {  // this rank's own share stays on the device
       if (sc) {
-        XCU(cudaMemcpyAsync(d_recv + roff[q], d_send + so, sc * sizeof(PpRecord), cudaMemcpyDeviceToDevice, st));
-        if (bc) XCU(cudaMemcpyAsync(d_recvbc + roff[q], d_sendbc + so, sc * 8, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(d_recv + roff[q], d_send + so, sc * sizeof(PpRecord), cudaMemcpyDeviceToDevice, st));
+        if (bc) CU(cudaMemcpyAsync(d_recvbc + roff[q], d_sendbc + so, sc * 8, cudaMemcpyDeviceToDevice, st));
       }
       continue;
     }
     if (sc) {
-      XNC(N.Send(d_send + so, sc * sizeof(PpRecord), NCCL_UINT8, q, ctx->nccl_comm, st));
-      if (bc) XNC(N.Send(d_sendbc + so, sc * 8, NCCL_UINT8, q, ctx->nccl_comm, st));
+      NC(N.Send(d_send + so, sc * sizeof(PpRecord), NCCL_UINT8, q, ctx->nccl_comm, st));
+      if (bc) NC(N.Send(d_sendbc + so, sc * 8, NCCL_UINT8, q, ctx->nccl_comm, st));
     }
     if (rc) {
-      XNC(N.Recv(d_recv + roff[q], rc * sizeof(PpRecord), NCCL_UINT8, q, ctx->nccl_comm, st));
-      if (bc) XNC(N.Recv(d_recvbc + roff[q], rc * 8, NCCL_UINT8, q, ctx->nccl_comm, st));
+      NC(N.Recv(d_recv + roff[q], rc * sizeof(PpRecord), NCCL_UINT8, q, ctx->nccl_comm, st));
+      if (bc) NC(N.Recv(d_recvbc + roff[q], rc * 8, NCCL_UINT8, q, ctx->nccl_comm, st));
     }
   }
-  XNC(N.GroupEnd());
-  XCU(cudaEventRecord(ev[2], st));
+  NC(N.GroupEnd());
+  CU(cudaEventRecord(ev[2], st));
   // ---- the ordinary single-GPU post-processing of what arrived
   PpParams P;
   P.kind = bc ? PP_BED_BC : PP_BED; P.low_mem = 1; P.dedup = p.remove_pcr_duplicates; P.tn5 = p.tn5_shift; P.mapq_threshold = p.mapq_threshold; P.se = 0;
   u64 nsel = 0;
   const int prc = pp_device(ctx, P, d_recv, d_recvbc, n_recv, d_res, d_resbc, &nsel);
-  if (prc != CMX_OK) { cleanup(); return prc; }
-  XCU(cudaEventRecord(ev[3], st));
+  if (prc != CMX_OK) return prc;
+  CU(cudaEventRecord(ev[3], st));
   *n_out = nsel;
-  if (nsel > out_capacity) { cleanup(); return fail(ctx, CMX_ERR_INVALID, "cmx_dedup_shuffle: %llu records for a capacity of %llu", (unsigned long long)nsel, (unsigned long long)out_capacity); }
+  if (nsel > out_capacity) return fail(ctx, CMX_ERR_INVALID, "cmx_dedup_shuffle: %llu records for a capacity of %llu", (unsigned long long)nsel, (unsigned long long)out_capacity);
   if (nsel) {
     const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    XCU(cudaMemcpyAsync(out_records, d_res, nsel * sizeof(PpRecord), kind, st));
-    if (bc && out_barcode_keys) XCU(cudaMemcpyAsync(out_barcode_keys, d_resbc, nsel * 8, kind, st));
+    CU(cudaMemcpyAsync(out_records, d_res, nsel * sizeof(PpRecord), kind, st));
+    if (bc && out_barcode_keys) CU(cudaMemcpyAsync(out_barcode_keys, d_resbc, nsel * 8, kind, st));
   }
-  XCU(cudaStreamSynchronize(st));
-  XCU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
   if (stats) {
     cudaEventElapsedTime(&stats->partition_ms, ev[0], ev[1]);
     cudaEventElapsedTime(&stats->shuffle_ms, ev[1], ev[2]);
@@ -1879,9 +1812,6 @@ int cmx_dedup_shuffle(cmx_ctx *ctx, const void *records, const uint64_t *barcode
     stats->bytes_sent = (n - cnt(rank, rank)) * rb; stats->bytes_received = (n_recv - cnt(rank, rank)) * rb;
     stats->n_received = n_recv; stats->n_global = n_global; stats->n_ranks = (uint32_t)R;
   }
-#undef XCU
-#undef XNC
-  cleanup();
   return CMX_OK;
 }
 
@@ -1903,59 +1833,101 @@ int cmx_exchange_finish(const cmx_params *params, cmx_pe_record *recs, uint64_t 
 // BED text on the device (bed_len_kernel / bed_write_kernel), byte-identical to cmx_format_bed / cmx_format_bed_bc.
 // Records (and barcode keys, NULL for bulk data) and the output buffer are host memory; work goes through the device in
 // chunks of 8 M records.  buf == NULL: returns the text length only.  Returns < 0 on error.
-int64_t cmx_format_bed_gpu(cmx_ctx *ctx, const char *const *names, const cmx_pe_record *records, const uint64_t *barcode_keys, uint64_t n,
-                           uint32_t bc_len, char *buf, int64_t cap) {
-  if (!ctx || !names || (!records && n) || (barcode_keys && (bc_len == 0 || bc_len > 32))) return -1;
-  if (cudaSetDevice(ctx->device) != cudaSuccess) return -1;
+static int format_bed_gpu(cmx_ctx *ctx, const char *const *names, const cmx_pe_record *records, const uint64_t *barcode_keys, uint64_t n,
+                          uint32_t bc_len, char *buf, int64_t cap, int64_t *total) {
   const u32 n_seq = ctx->n_seq;
   std::string cat;
   std::vector<u32> noff(n_seq + 1, 0);
   for (u32 i = 0; i < n_seq; ++i) { cat += names[i]; noff[i + 1] = (u32)cat.size(); }
   const u64 CH = 8u << 20;
   const u64 nc = std::min<u64>(n, CH);
-  char *d_names = nullptr, *d_out = nullptr;
-  u32 *d_noff = nullptr, *d_len = nullptr;
-  PpRecord *d_rec = nullptr;
-  u64 *d_bc = nullptr, *d_off = nullptr;
-  void *d_tmp = nullptr;
-  size_t out_cap = 0, tmp_bytes = 0;
-  int64_t total = 0;
-  bool ok = true;
-  auto CK = [&](cudaError_t e) { if (e != cudaSuccess) { ok = false; ctx->err = std::string("cmx_format_bed_gpu: ") + cudaGetErrorString(e); } return ok; };
+  DevMem<char> d_names, d_out;
+  DevMem<u32> d_noff, d_len;
+  DevMem<PpRecord> d_rec;
+  DevMem<u64> d_bc, d_off;
+  DevMem<> d_tmp;
+  size_t tmp_bytes = 0;
   cudaStream_t st = ctx->stream;
-  do {
-    if (!CK(cudaMalloc(&d_names, cat.size() + 1)) || !CK(cudaMalloc(&d_noff, (n_seq + 1) * 4))) break;
-    if (!CK(cudaMemcpyAsync(d_names, cat.data(), cat.size(), cudaMemcpyHostToDevice, st)) || !CK(cudaMemcpyAsync(d_noff, noff.data(), (n_seq + 1) * 4, cudaMemcpyHostToDevice, st))) break;
-    if (nc == 0) break;
-    if (!CK(cudaMalloc(&d_rec, nc * sizeof(PpRecord))) || !CK(cudaMalloc(&d_len, (nc + 1) * 4)) || !CK(cudaMalloc(&d_off, (nc + 1) * 8))) break;
-    if (barcode_keys && !CK(cudaMalloc(&d_bc, nc * 8))) break;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_len, d_off, (int)nc + 1, st);
-    if (!CK(cudaMalloc(&d_tmp, tmp_bytes))) break;
-    for (u64 c0 = 0; c0 < n && ok; c0 += CH) {
-      const u64 m = std::min(CH, n - c0);
-      const unsigned nb = (unsigned)((m + 255) / 256);
-      if (!CK(cudaMemcpyAsync(d_rec, records + c0, m * sizeof(PpRecord), cudaMemcpyHostToDevice, st))) break;
-      if (barcode_keys && !CK(cudaMemcpyAsync(d_bc, barcode_keys + c0, m * 8, cudaMemcpyHostToDevice, st))) break;
-      if (!CK(cudaMemsetAsync(d_len + m, 0, 4, st))) break;
-      bed_len_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_noff, barcode_keys ? (int)bc_len : 0, d_len);
-      if (!CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_len, d_off, (int)m + 1, st))) break;
-      u64 bytes = 0;
-      if (!CK(cudaMemcpyAsync(&bytes, d_off + m, 8, cudaMemcpyDeviceToHost, st)) || !CK(cudaStreamSynchronize(st))) break;
-      if (buf && total + (int64_t)bytes <= cap) {
-        if (bytes > out_cap) { cudaFree(d_out); d_out = nullptr; out_cap = bytes + bytes / 8; if (!CK(cudaMalloc(&d_out, out_cap))) break; }
-        bed_write_kernel<<<nb, 256, 0, st>>>(d_rec, d_bc, m, d_names, d_noff, barcode_keys ? (int)bc_len : 0, d_off, 0, d_out);
-        if (!CK(cudaMemcpyAsync(buf + total, d_out, bytes, cudaMemcpyDeviceToHost, st)) || !CK(cudaStreamSynchronize(st))) break;
-      }
-      total += (int64_t)bytes;
+  CU(d_names.alloc(cat.size() + 1)); CU(d_noff.alloc((n_seq + 1) * 4));
+  CU(cudaMemcpyAsync(d_names, cat.data(), cat.size(), cudaMemcpyHostToDevice, st)); CU(cudaMemcpyAsync(d_noff, noff.data(), (n_seq + 1) * 4, cudaMemcpyHostToDevice, st));
+  if (nc == 0) { CU(cudaGetLastError()); return CMX_OK; }
+  CU(d_rec.alloc(nc * sizeof(PpRecord))); CU(d_len.alloc((nc + 1) * 4)); CU(d_off.alloc((nc + 1) * 8));
+  if (barcode_keys) CU(d_bc.alloc(nc * 8));
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_len.p, d_off.p, (int)nc + 1, st);
+  CU(d_tmp.alloc(tmp_bytes));
+  for (u64 c0 = 0; c0 < n; c0 += CH) {
+    const u64 m = std::min(CH, n - c0);
+    const unsigned nb = (unsigned)((m + 255) / 256);
+    CU(cudaMemcpyAsync(d_rec, records + c0, m * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
+    if (barcode_keys) CU(cudaMemcpyAsync(d_bc, barcode_keys + c0, m * 8, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(d_len + m, 0, 4, st));
+    bed_len_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_noff, barcode_keys ? (int)bc_len : 0, d_len);
+    CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_len.p, d_off.p, (int)m + 1, st));
+    u64 bytes = 0;
+    CU(cudaMemcpyAsync(&bytes, d_off + m, 8, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
+    if (buf && *total + (int64_t)bytes <= cap) {
+      if (bytes > d_out.cap) CU(d_out.alloc(bytes + bytes / 8));  // (alloc frees the smaller buffer first)
+      bed_write_kernel<<<nb, 256, 0, st>>>(d_rec, d_bc, m, d_names, d_noff, barcode_keys ? (int)bc_len : 0, d_off, 0, d_out);
+      CU(cudaMemcpyAsync(buf + *total, d_out, bytes, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
     }
-  } while (0);
-  if (ok) CK(cudaGetLastError());
-  cudaFree(d_names); cudaFree(d_noff); cudaFree(d_rec); cudaFree(d_len); cudaFree(d_off); cudaFree(d_bc); cudaFree(d_tmp); cudaFree(d_out);
-  return ok ? total : -1;
+    *total += (int64_t)bytes;
+  }
+  CU(cudaGetLastError());
+  return CMX_OK;
+}
+int64_t cmx_format_bed_gpu(cmx_ctx *ctx, const char *const *names, const cmx_pe_record *records, const uint64_t *barcode_keys, uint64_t n,
+                           uint32_t bc_len, char *buf, int64_t cap) {
+  if (!ctx || !names || (!records && n) || (barcode_keys && (bc_len == 0 || bc_len > 32))) return -1;
+  if (cudaSetDevice(ctx->device) != cudaSuccess) return -1;
+  int64_t total = 0;
+  return format_bed_gpu(ctx, names, records, barcode_keys, n, bc_len, buf, cap, &total) == CMX_OK ? total : -1;
 }
 
 // Pairs text on the device (pairs_len_kernel / pairs_write_kernel), byte-identical to cmx_format_pairs: the header is
 // written by the host, the lines by one thread each.  Read names travel as one concatenation + offsets.
+static int format_pairs_gpu(cmx_ctx *ctx, const char *const *names, uint32_t n_seq, const cmx_pairs_record *records, uint64_t n,
+                            const char *const *read_names, uint64_t n_read_names, uint32_t first_read_id, char *buf, int64_t cap, int64_t *total) {
+  std::string cat;
+  std::vector<u32> noff(n_seq + 1, 0);
+  for (u32 i = 0; i < n_seq; ++i) { cat += names[i]; noff[i + 1] = (u32)cat.size(); }
+  std::vector<u64> roff(n_read_names + 1, 0);
+  for (u64 i = 0; i < n_read_names; ++i) roff[i + 1] = roff[i] + strlen(read_names[i]);
+  std::string rcat;
+  rcat.resize(roff[n_read_names]);
+  for (u64 i = 0; i < n_read_names; ++i) memcpy(&rcat[roff[i]], read_names[i], roff[i + 1] - roff[i]);
+  DevMem<char> d_names, d_rn, d_out;
+  DevMem<u32> d_noff, d_len;
+  DevMem<u64> d_roff, d_off;
+  DevMem<PpRecord> d_rec;
+  DevMem<> d_tmp;
+  size_t tmp_bytes = 0;
+  cudaStream_t st = ctx->stream;
+  const u64 CH = 8u << 20;
+  const u64 nc = std::min<u64>(n, CH);
+  CU(d_names.alloc(cat.size() + 1)); CU(d_noff.alloc((n_seq + 1) * 4)); CU(d_rn.alloc(rcat.size() + 1));
+  CU(d_roff.alloc((n_read_names + 1) * 8)); CU(d_rec.alloc(nc * sizeof(PpRecord))); CU(d_len.alloc((nc + 1) * 4)); CU(d_off.alloc((nc + 1) * 8));
+  CU(cudaMemcpyAsync(d_names, cat.data(), cat.size(), cudaMemcpyHostToDevice, st)); CU(cudaMemcpyAsync(d_noff, noff.data(), (n_seq + 1) * 4, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_rn, rcat.data(), rcat.size(), cudaMemcpyHostToDevice, st)); CU(cudaMemcpyAsync(d_roff, roff.data(), (n_read_names + 1) * 8, cudaMemcpyHostToDevice, st));
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_len.p, d_off.p, (int)nc + 1, st);
+  CU(d_tmp.alloc(tmp_bytes));
+  for (u64 c0 = 0; c0 < n; c0 += CH) {
+    const u64 m = std::min(CH, n - c0);
+    const unsigned nb = (unsigned)((m + 255) / 256);
+    CU(cudaMemcpyAsync(d_rec, records + c0, m * sizeof(PpRecord), cudaMemcpyHostToDevice, st)); CU(cudaMemsetAsync(d_len + m, 0, 4, st));
+    pairs_len_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_noff, d_roff, first_read_id, d_len);
+    CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_len.p, d_off.p, (int)m + 1, st));
+    u64 bytes = 0;
+    CU(cudaMemcpyAsync(&bytes, d_off + m, 8, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
+    if (buf && *total + (int64_t)bytes <= cap) {
+      if (bytes > d_out.cap) CU(d_out.alloc(bytes + bytes / 8));  // (alloc frees the smaller buffer first)
+      pairs_write_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_names, d_noff, d_rn, d_roff, first_read_id, d_off, d_out);
+      CU(cudaMemcpyAsync(buf + *total, d_out, bytes, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
+    }
+    *total += (int64_t)bytes;
+  }
+  CU(cudaGetLastError());
+  return CMX_OK;
+}
 int64_t cmx_format_pairs_gpu(cmx_ctx *ctx, const char *const *names, const uint32_t *lengths, uint32_t n_seq, const cmx_pairs_record *records, uint64_t n,
                              const char *const *read_names, uint64_t n_read_names, uint32_t first_read_id, char *buf, int64_t cap) {
   if (!ctx || !names || !lengths || (!records && n) || (!read_names && n)) return -1;
@@ -1966,55 +1938,7 @@ int64_t cmx_format_pairs_gpu(cmx_ctx *ctx, const char *const *names, const uint3
   int64_t total = (int64_t)hdr.size();
   if (buf && total <= cap) memcpy(buf, hdr.data(), hdr.size());
   if (n == 0) return total;
-  std::string cat;
-  std::vector<u32> noff(n_seq + 1, 0);
-  for (u32 i = 0; i < n_seq; ++i) { cat += names[i]; noff[i + 1] = (u32)cat.size(); }
-  std::vector<u64> roff(n_read_names + 1, 0);
-  for (u64 i = 0; i < n_read_names; ++i) roff[i + 1] = roff[i] + strlen(read_names[i]);
-  std::string rcat;
-  rcat.resize(roff[n_read_names]);
-  for (u64 i = 0; i < n_read_names; ++i) memcpy(&rcat[roff[i]], read_names[i], roff[i + 1] - roff[i]);
-  char *d_names = nullptr, *d_rn = nullptr, *d_out = nullptr;
-  u32 *d_noff = nullptr, *d_len = nullptr;
-  u64 *d_roff = nullptr, *d_off = nullptr;
-  PpRecord *d_rec = nullptr;
-  void *d_tmp = nullptr;
-  size_t tmp_bytes = 0;
-  bool ok = true;
-  auto CK = [&](cudaError_t e) { if (e != cudaSuccess) { ok = false; ctx->err = std::string("cmx_format_pairs_gpu: ") + cudaGetErrorString(e); } return ok; };
-  cudaStream_t st = ctx->stream;
-  const u64 CH = 8u << 20;
-  const u64 nc = std::min<u64>(n, CH);
-  do {
-    if (!CK(cudaMalloc(&d_names, cat.size() + 1)) || !CK(cudaMalloc(&d_noff, (n_seq + 1) * 4)) || !CK(cudaMalloc(&d_rn, rcat.size() + 1)) ||
-        !CK(cudaMalloc(&d_roff, (n_read_names + 1) * 8)) || !CK(cudaMalloc(&d_rec, nc * sizeof(PpRecord))) || !CK(cudaMalloc(&d_len, (nc + 1) * 4)) ||
-        !CK(cudaMalloc(&d_off, (nc + 1) * 8)))
-      break;
-    if (!CK(cudaMemcpyAsync(d_names, cat.data(), cat.size(), cudaMemcpyHostToDevice, st)) || !CK(cudaMemcpyAsync(d_noff, noff.data(), (n_seq + 1) * 4, cudaMemcpyHostToDevice, st)) ||
-        !CK(cudaMemcpyAsync(d_rn, rcat.data(), rcat.size(), cudaMemcpyHostToDevice, st)) || !CK(cudaMemcpyAsync(d_roff, roff.data(), (n_read_names + 1) * 8, cudaMemcpyHostToDevice, st)))
-      break;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_len, d_off, (int)nc + 1, st);
-    if (!CK(cudaMalloc(&d_tmp, tmp_bytes))) break;
-    size_t out_cap = 0;
-    for (u64 c0 = 0; c0 < n && ok; c0 += CH) {
-      const u64 m = std::min(CH, n - c0);
-      const unsigned nb = (unsigned)((m + 255) / 256);
-      if (!CK(cudaMemcpyAsync(d_rec, records + c0, m * sizeof(PpRecord), cudaMemcpyHostToDevice, st)) || !CK(cudaMemsetAsync(d_len + m, 0, 4, st))) break;
-      pairs_len_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_noff, d_roff, first_read_id, d_len);
-      if (!CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_len, d_off, (int)m + 1, st))) break;
-      u64 bytes = 0;
-      if (!CK(cudaMemcpyAsync(&bytes, d_off + m, 8, cudaMemcpyDeviceToHost, st)) || !CK(cudaStreamSynchronize(st))) break;
-      if (buf && total + (int64_t)bytes <= cap) {
-        if (bytes > out_cap) { cudaFree(d_out); d_out = nullptr; out_cap = bytes + bytes / 8; if (!CK(cudaMalloc(&d_out, out_cap))) break; }
-        pairs_write_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_names, d_noff, d_rn, d_roff, first_read_id, d_off, d_out);
-        if (!CK(cudaMemcpyAsync(buf + total, d_out, bytes, cudaMemcpyDeviceToHost, st)) || !CK(cudaStreamSynchronize(st))) break;
-      }
-      total += (int64_t)bytes;
-    }
-  } while (0);
-  if (ok) CK(cudaGetLastError());
-  cudaFree(d_names); cudaFree(d_noff); cudaFree(d_rn); cudaFree(d_roff); cudaFree(d_rec); cudaFree(d_len); cudaFree(d_off); cudaFree(d_tmp); cudaFree(d_out);
-  return ok ? total : -1;
+  return format_pairs_gpu(ctx, names, n_seq, records, n, read_names, n_read_names, first_read_id, buf, cap, &total) == CMX_OK ? total : -1;
 }
 
 // --TagAlign for paired-end records (mapping_writer.cc:84-110): one line per mate, the duplicate count on the second.
