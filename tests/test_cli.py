@@ -75,6 +75,30 @@ def test_index_file_written_by_cli_is_loadable_by_the_reference_binary(tmp_path,
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("case,index_args,args", [("mfl100_q0", ["--min-frag-length", "100"], ["-q", "0"]), ("mfl70", ["-k", "19", "-w", "10"], [])])
+def test_cli_index_shapes_equal_reference_binary_output(case, index_args, args, tmp_path, golden_dir):
+    """`-i --min-frag-length 100` picks (23, 11) and `-i -k 19 -w 10` builds (19, 10), as the reference does; mapping on them
+    gives the reference binary's BED.  The (23, 11) index file is also loadable by the reference binary, with the same BED."""
+    cli = _ensure_cli()
+    d = os.path.join(golden_dir, "synth_small")
+    idx = str(tmp_path / "ref.index")
+    subprocess.check_call([cli, "-i"] + index_args + ["-r", os.path.join(d, "ref.fa.gz"), "-o", idx], stderr=subprocess.DEVNULL)
+    want = gzip.open(os.path.join(golden_dir, "synth_params", case + ".bed.gz")).read()
+    out = str(tmp_path / "out.bed")
+    subprocess.check_call([cli] + args + ["-x", idx, "-r", os.path.join(d, "ref.fa.gz"), "-1", os.path.join(d, "read1.fq.gz"),
+                                         "-2", os.path.join(d, "read2.fq.gz"), "-o", out], stderr=subprocess.DEVNULL)
+    assert open(out, "rb").read() == want
+    if case != "mfl100_q0":
+        return
+    if not os.path.exists(REF_BIN):
+        pytest.skip("oracle/_ref/chromap not built")
+    ref_out = str(tmp_path / "ref_out.bed")
+    subprocess.check_call([REF_BIN] + args + ["-x", idx, "-r", os.path.join(d, "ref.fa.gz"), "-1", os.path.join(d, "read1.fq.gz"),
+                                             "-2", os.path.join(d, "read2.fq.gz"), "-o", ref_out, "-t", "2"], stderr=subprocess.DEVNULL)
+    assert open(ref_out, "rb").read() == want
+
+
+@pytest.mark.gpu
 def test_cli_hic_preset_pairs_output(tmp_path, golden_dir):
     cli = _ensure_cli()
     d = os.path.join(golden_dir, "synth_hic")

@@ -15,7 +15,10 @@ some of them up to the last tier (512-thread pair_candidates_cta, 256-thread ver
 trimming by prep_kernel on read-through pairs); `--preset hic` (split alignment: verify_split / pairing_split / emit_split and the
 CTA form, chimeric reads, pairs records); single-end (emit_se_kernel, a fresh generator per read), each also through the CTA tiers; `--SAM` (emit_sam_kernel: spans and CIGARs by
 the diagonal-band aligner, against the oracle's SAM cores); a 420-copy repeat family (thousands of hits and hundreds of candidates per
-read, the real capacities up to the last tier)."""
+read, the real capacities up to the last tier).  The whole pipeline also runs at index shapes (19, 10), (23, 11) (k > 22: no
+shared-memory key buffer in the front end; chip, CTA tiers, single-end, SAM, Hi-C), (28, 20) and (16, 5), and at mapping knobs
+off their defaults: -e 1 / 7 / 15, -n 8 through the CTA tiers, -s 1, -f low enough for repetitive seeds and the second seeding
+round, --drop-repetitive-reads and --min-read-length."""
 import os
 import re
 import subprocess
@@ -62,7 +65,10 @@ static std::string revc(const std::string &s) { std::string r(s.rbegin(), s.rend
 struct RunStats { long pairs = 0, records = 0, tier_pairs[3] = {0, 0, 0}, bad = 0; };
 
 enum { MODE_CHIP = 0, MODE_ATAC = 1, MODE_HIC = 2, MODE_SE = 3, MODE_SAM = 4, MODE_SAM_SE = 5 };
-static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *caps3, int max_best, int read_len_base, bool front_only = false, int K = 17, int W = 7, int fam_copies = 90) {
+// mapping knobs over the preset (-1: the preset's value): -e, -s, -f f0,f1, --drop-repetitive-reads, --min-read-length
+struct Knobs { int e = -1, min_seeds = -1, f0 = -1, f1 = -1, drop_rep = -1, min_read_len = -1; };
+static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *caps3, int max_best, int read_len_base, bool front_only = false, int K = 17, int W = 7, int fam_copies = 90,
+                         const Knobs &kn = Knobs{}) {
   std::mt19937 g((unsigned)seed);
   RunStats rs;
   // ---- reference: two sequences, a 300 bp family with many copies, a 2 kb segmental repeat, an N run
@@ -124,6 +130,12 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   // ---- oracle
   orc_params op; orc_default_params(&op); orc_apply_preset(&op, mode == MODE_ATAC ? "atac" : mode == MODE_HIC ? "hic" : "chip");
   op.max_num_best_mappings = max_best;
+  if (kn.e >= 0) op.error_threshold = kn.e;
+  if (kn.min_seeds >= 0) op.min_num_seeds = kn.min_seeds;
+  if (kn.f0 >= 0) op.max_seed_freq0 = kn.f0;
+  if (kn.f1 >= 0) op.max_seed_freq1 = kn.f1;
+  if (kn.drop_rep >= 0) op.drop_repetitive_reads = kn.drop_rep;
+  if (kn.min_read_len >= 0) op.min_read_length = kn.min_read_len;
   const bool is_se = mode == MODE_SE || mode == MODE_SAM_SE, is_sam = mode == MODE_SAM || mode == MODE_SAM_SE;
   op.single_end = is_se;
   orc_mapper *om = orc_mapper_create(&op, oix, oref);
@@ -222,7 +234,7 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
       }
       std::vector<int> vlist((size_t)2 * n_slots + 8), rlist((size_t)n_slots + 8);
       int d_count[4] = {0, 0, 0, 0};
-      int rows0 = (2 * mrl / (7 + 1) + 15) / 16 * 16;
+      int rows0 = (2 * mrl / (W + 1) + 15) / 16 * 16;
       rows0 = std::max(16, std::min(rows0, S.caps.hc));
       launch((2 * n_slots + CLUSTER_NT - 1) / CLUSTER_NT, CLUSTER_NT, (size_t)rows0 * CLUSTER_NT * 8, [&]() { cluster_kernel(P, ix, S, &ctr, 0, rows0, vlist.data(), &d_count[3]); });
       if (rows0 < S.caps.hc)
@@ -336,7 +348,7 @@ int main() {
   const Caps small[3] = {{mrl, 6, 2, 2}, {mrl * 2, 40, 6, 6}, {mrl * 4, 65536, 8192, 8192}};            // most pairs through the CTA kernels, some to the last tier
   const Caps real_long[3] = {{150, 64, 32, 32}, {300, 1024, 256, 256}, {600, 65536, 8192, 8192}};
   const Caps small_long[3] = {{150, 6, 2, 2}, {300, 40, 6, 6}, {600, 65536, 8192, 8192}};
-  struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; };
+  struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; Knobs knobs = {}; };
   const Case cases[] = {
       {"real_tiers", MODE_CHIP, 3, 100, 1, 60, real, mrl},
       {"small_first_tier", MODE_CHIP, 4, 48, 3, 60, small, mrl},
@@ -351,10 +363,36 @@ int main() {
       {"front_end_only", MODE_CHIP, 11, 600, 1, 60, real, mrl, true},
       {"front_end_k21_w10", MODE_CHIP, 12, 200, 1, 60, real, mrl, true, 21, 10},     // the run-time scan (seed_front_kernel<false>)
       {"front_end_k16_w5", MODE_CHIP, 13, 200, 1, 60, real, mrl, true, 16, 5},       // even k: strand-symmetric k-mers
+      // other index shapes, the whole pipeline: the run-time scan, k - 1 shifts of reverse-strand candidates, k + w - 1 overlaps
+      // of repetitive seeds, the first cluster pass's rows by w.  For k > 22 the front end keeps every minimizer in the record arrays.
+      {"k19_w10", MODE_CHIP, 16, 80, 1, 60, real, mrl, false, 19, 10},
+      {"k19_w10_cta", MODE_CHIP, 17, 40, 2, 60, small, mrl, false, 19, 10},
+      {"k23_w11", MODE_CHIP, 18, 80, 1, 60, real, mrl, false, 23, 11},
+      {"k23_w11_cta", MODE_CHIP, 19, 40, 2, 60, small, mrl, false, 23, 11},
+      {"k23_w11_single_end", MODE_SE, 20, 50, 2, 60, real, mrl, false, 23, 11},
+      {"k23_w11_sam", MODE_SAM, 21, 40, 2, 60, real, mrl, false, 23, 11},
+      {"k23_w11_hic", MODE_HIC, 22, 30, 1, 120, real_long, 150, false, 23, 11},
+      {"k28_w20", MODE_CHIP, 23, 60, 1, 60, real, mrl, false, 28, 20},
+      {"k16_w5", MODE_CHIP, 24, 60, 1, 60, real, mrl, false, 16, 5},
+      // repetitive seeds at w > k: gaps between minimizers reach past k + 6, so the k + w - 1 overlap rule matters; MAPQ shows it
+      // for uniquely mapped reads that run into a repeat copy
+      {"k14_w30_repetitive", MODE_CHIP, 25, 100, 1, 120, real_long, 150, false, 14, 30, 90, Knobs{.f0 = 3, .f1 = 40}},
+      {"k14_w30_repetitive_se", MODE_SE, 35, 100, 1, 120, real_long, 150, false, 14, 30, 90, Knobs{.f0 = 3, .f1 = 40}},
+      // mapping knobs: error thresholds at both ends and across the 8 / 4 lane boundary, -n 8 through the CTA tiers, -s, -f low
+      // enough for the second seeding round and repetitive-seed MAPQ, --drop-repetitive-reads, --min-read-length inside the read lengths
+      {"e1", MODE_CHIP, 26, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.e = 1}},
+      {"e7", MODE_CHIP, 27, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.e = 7}},
+      {"e15", MODE_CHIP, 28, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.e = 15}},
+      {"e15_cta", MODE_CHIP, 29, 30, 2, 60, small, mrl, false, 17, 7, 90, Knobs{.e = 15}},
+      {"n8_cta", MODE_CHIP, 30, 40, 8, 60, small, mrl},
+      {"s1", MODE_CHIP, 31, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.min_seeds = 1}},
+      {"f3_40", MODE_CHIP, 32, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.f0 = 3, .f1 = 40}},
+      {"drop20", MODE_CHIP, 33, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.drop_rep = 20}},
+      {"min_read_length58", MODE_CHIP, 34, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.min_read_len = 58}},
   };
   const int seed_off = getenv("EMU_SEED_OFFSET") ? atoi(getenv("EMU_SEED_OFFSET")) : 0;   // other inputs of the same kinds (offline fuzzing)
   for (const Case &c : cases) {
-    const RunStats r = run_case(c.mode, c.seed + seed_off, c.n, c.mrl, c.caps, c.max_best, c.len, c.front_only, c.k, c.w, c.fam_copies);
+    const RunStats r = run_case(c.mode, c.seed + seed_off, c.n, c.mrl, c.caps, c.max_best, c.len, c.front_only, c.k, c.w, c.fam_copies, c.knobs);
     printf("%%s: pairs=%%ld records=%%ld tier0=%%ld tier1=%%ld tier2=%%ld bad=%%ld\n", c.name, r.pairs, r.records, r.tier_pairs[0], r.tier_pairs[1], r.tier_pairs[2], r.bad);
     bad += r.bad;
   }
@@ -389,3 +427,10 @@ def test_device_pipeline_on_emulated_ctas_equals_the_oracle(tmp_path):
     assert got["small_first_tier"][1] > 30 and got["small_first_tier"][3] > 20 and got["small_first_tier"][4] > 3, out.stdout   # CTA kernels, up to the last tier
     assert got["atac_trimming"][1] > 20 and got["hic_split"][1] > 18 and got["single_end"][1] > 25, out.stdout
     assert got["hic_split_cta"][3] > 3 and got["single_end_cta"][3] > 6 and got["sam_cores"][1] > 25 and got["sam_cores_single_end"][1] > 20 and got["heavy_repeats"][4] > 3 and got["front_end_only"][1] > 5000 and got["front_end_k21_w10"][1] > 800 and got["front_end_k16_w5"][1] > 1500, out.stdout
+    # other index shapes and knobs: (records, pairs in the second tier, pairs in the last tier) at least
+    floors = {"k19_w10": (50, 10, 0), "k19_w10_cta": (30, 15, 8), "k23_w11": (40, 12, 0), "k23_w11_cta": (25, 15, 8), "k23_w11_single_end": (35, 5, 0),
+              "k23_w11_sam": (25, 5, 0), "k23_w11_hic": (18, 8, 0), "k28_w20": (15, 5, 0), "k16_w5": (40, 8, 0), "k14_w30_repetitive": (55, 0, 0), "k14_w30_repetitive_se": (50, 0, 0),
+              "e1": (8, 12, 0), "e7": (30, 12, 0), "e15": (40, 12, 0), "e15_cta": (25, 15, 8), "n8_cta": (60, 15, 8), "s1": (40, 12, 0),
+              "f3_40": (30, 4, 0), "drop20": (30, 10, 0), "min_read_length58": (18, 10, 0)}
+    for name, (records, tier1, tier2) in floors.items():
+        assert got[name][1] > records and got[name][3] >= tier1 and got[name][4] >= tier2, (name, out.stdout)
