@@ -23,6 +23,11 @@ inline void mapq_tables_fill(double *inv_log, int *pen_thr) {
     pen_thr[v] = (int)lo;
   }
 }
+// select_kernel's mt_init: the 624-word state of std::mt19937(11) right after seeding.
+inline void mt_init_fill(u32 *mt) {
+  mt[0] = 11u;
+  for (int i = 1; i < 624; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (u32)i;
+}
 
 struct Counters {  // device-side statistics (atomics)
   u64 n_minimizers, n_probe_steps, n_found, n_occ_reads, n_verified, n_candidates, n_mapped, n_unique, n_overflow;

@@ -12,7 +12,7 @@ ORACLE_LIB = os.path.join(ROOT, "oracle", "liboracle.so")
 
 # the mapping pipeline, in include order
 PIPELINE = ["device_common.cuh", "minimizers.cuh", "pipeline_kernels.cuh", "seed_front.cuh", "cta_pair_candidates.cuh", "cta_verify_pairing.cuh",
-            "sam_kernels.cuh"]
+            "sam_kernels.cuh", "lane_pipeline.cuh"]
 
 
 def source(headers):

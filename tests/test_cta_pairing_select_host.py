@@ -69,8 +69,7 @@ int main() {
   }
   // ---- multi-mapper sampling
   u32 mt_init[624];
-  mt_init[0] = 11u;
-  for (int i = 1; i < 624; ++i) mt_init[i] = 1812433253u * (mt_init[i - 1] ^ (mt_init[i - 1] >> 30)) + (u32)i;   // std::mt19937(11) right after seeding
+  mt_init_fill(mt_init);
   for (int it = 0; it < 12; ++it) {
     DevParams P{};
     P.max_best = 1 + (int)(g() %% 8); P.se = it %% 10 == 9;

@@ -2,9 +2,9 @@
 seed_cta -> pair_candidates_cta -> verify_cta -> pairing_cta (overflow tiers, one CTA per read / pair), overflow collection
 between the tiers, select, emit (+ deferred tracebacks) / emit_cta — compiled from the UNCHANGED kernel sources
 (device_common.cuh, minimizers.cuh, pipeline_kernels.cuh, seed_front.cuh, cta_pair_candidates.cuh, cta_verify_pairing.cuh, sam_kernels.cuh) and run on the host
-emulation of CTAs (tests/cta_emu.h) with the launch sequence, grid / block sizes, shared-memory sizes and scratch layout of
-the library's run_lane (the layout by the library's own `scratch_layout`), against the oracle's mapper (`orc_map_pairs`, pinned to the
-reference binary by tests/test_oracle_golden.py): every pair's records, field by field.
+emulation of CTAs (tests/cta_emu.h) by the library's own launch sequence (lane_pipeline.cuh: kernel order, grid / block and
+shared-memory sizes, the host decisions between the kernels) and scratch layout (`scratch_layout`), against the oracle's mapper
+(`orc_map_pairs`, pinned to the reference binary by tests/test_oracle_golden.py): every pair's records, field by field.
 The front end runs too (seed_front_kernel: persistent grid, double-buffered read tiles, packed-key minimizer scan, table probes,
 lane-interleaved records): only its six PTX wrappers (mbarrier.* / cp.async.bulk) are replaced by cta_emu.h's host equivalents —
 an mbarrier word with byte and arrival counts, a copy that signals its bytes — and its records are also compared one by one with
@@ -34,7 +34,6 @@ struct HostTier {
   std::vector<char> mem;
   std::vector<std::vector<char>> parts;   // EMU_EXACT_SCRATCH: every scratch array its own exactly sized allocation (AddressSanitizer then sees overruns between them)
   Scratch view;
-  std::vector<int> list;   // pair list of this tier (empty = identity)
 };
 static void tier_prepare_host(HostTier &t, int n_slots, const int *pair_list, bool interleaved) {
   size_t o[SCRATCH_ARRAYS];
@@ -53,12 +52,31 @@ static void tier_prepare_host(HostTier &t, int n_slots, const int *pair_list, bo
   scratch_bind(S, a);
 }
 static std::vector<u64> g_smem;
-template <typename F>
-static void launch(int grid, int block, size_t smem_bytes, F body) {   // kernel<<<grid, block, smem>>>(...)
-  g_smem.assign(smem_bytes / 8 + 2, 0xA5A5A5A5A5A5A5A5ull);
-  g_dyn_smem = g_smem.data();
-  emu_grid(grid, block, body);
-}
+// The emulation's side of the library's launch sequence (lane_pipeline.cuh): a launch runs the grid's CTAs one after the
+// other.  Dynamic shared memory and the list buffers are fresh allocations of exactly the size asked for, so that
+// AddressSanitizer sees any access past them.
+struct EmuLane {
+  HostTier tiers[N_TIERS];
+  std::vector<char> lists[LIST_OVERFLOW + N_TIERS];
+  int cnt[4] = {0, 0, 0, 0};
+  std::vector<int> chunks;
+  template <typename... KA, typename... A>
+  void operator()(void (*kernel)(KA...), int grid, int block, size_t smem, A... a) {
+    g_smem = std::vector<u64>((smem + 7) / 8, 0xA5A5A5A5A5A5A5A5ull);
+    g_dyn_smem = g_smem.data();
+    emu_grid(grid, block, [&]() { kernel(a...); });
+  }
+  void mark(int) {}
+  void wait_piece(u32) {}
+  Scratch tier(int t, int n, const int *pair_list) { tier_prepare_host(tiers[t], n, pair_list, t == 0); return tiers[t].view; }
+  void *list(int l, size_t bytes) { lists[l] = std::vector<char>(bytes); return lists[l].data(); }
+  void clear_counts(int i, int n) { std::fill(cnt + i, cnt + i + n, 0); }
+  int overflow_count(int) { return cnt[0]; }
+  const int *sort_list(int *list, int n) { std::sort(list, list + n); return list; }
+  const int *chunk_starts(const std::vector<int> &c) { chunks = c; return chunks.data(); }
+  void emit_on(int) {}
+  void emit_join(int) {}
+};
 static char comp(char c) { switch (c) { case 'A': case 'a': return 'T'; case 'C': case 'c': return 'G'; case 'G': case 'g': return 'C'; case 'T': case 't': return 'A'; default: return 'N'; } }
 static std::string revc(const std::string &s) { std::string r(s.rbegin(), s.rend()); for (auto &c : r) c = comp(c); return r; }
 
@@ -147,10 +165,7 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   const long n_want = is_sam ? 0 : mode == MODE_SE ? (long)orc_map_reads_se(om, (u32)n, s1.data(), o1.data(), first_read_id, want.data(), (long)want.size(), 1)
                                       : (long)orc_map_pairs(om, (u32)n, s1.data(), o1.data(), s2.data(), o2.data(), first_read_id, want.data(), (long)want.size(), nullptr);
   // ---- device objects
-  DevParams P{};
-  P.e = op.error_threshold; P.min_seeds = op.min_num_seeds; P.f0 = op.max_seed_freq0; P.f1 = op.max_seed_freq1; P.max_best = max_best; P.max_insert = op.max_insert_size;
-  P.min_read_len = op.min_read_length; P.drop_rep = op.drop_repetitive_reads; P.trim = op.trim_adapters; P.k = K; P.w = W; P.lanes = P.e < 8 ? 8 : 4; P.split = op.split_alignment;
-  P.se = is_se;
+  const DevParams P = dev_params(op, K, W);
   const uint32_t *kf; const uint64_t *kk, *kv, *kocc; uint32_t n_occ = 0;
   const uint32_t nb = orc_index_arrays(oix, &kf, &kk, &kv, &kocc, &n_occ);
   // the library's table: 16-byte slots {hash << 1 | singleton, value}, slot = (hash * phi64) >> shift, linear probing, load <= 0.5
@@ -178,119 +193,52 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   mapq_tables_fill(il_.data(), thr_.data());
   MapqTables T{il_.data(), thr_.data()};
   u32 mt_init[624];
-  mt_init[0] = 11u;
-  for (int i = 1; i < 624; ++i) mt_init[i] = 1812433253u * (mt_init[i - 1] ^ (mt_init[i - 1] >> 30)) + (u32)i;
-  // ---- run_lane, tier by tier
-  HostTier tiers[3];
-  for (int t = 0; t < 3; ++t) tiers[t].caps = caps3[t];
+  mt_init_fill(mt_init);
+  // ---- run_lane's sequence
   Counters ctr{};
   std::vector<int> nbest((size_t)n, 0), sel((size_t)n * max_best, 0), out_n((size_t)n + 1, 0);
   std::vector<OutRecord> out_rec((size_t)n * max_best);
   std::vector<OutSam> out_sam(is_sam ? (size_t)n * max_best : 1);
   memset(out_sam.data(), 0, out_sam.size() * sizeof(OutSam));
-  int n_slots = n, tiers_used = 0;
-  const int *pair_list = nullptr;
-  const int TB = 128;
+  EmuLane x;
+  for (int t = 0; t < N_TIERS; ++t) x.tiers[t].caps = caps3[t];
+  const LaneArgs a{P, ix, R, B, T, mt_init, &ctr, x.cnt, nbest.data(), sel.data(), out_n.data(), is_sam ? (void *)out_sam.data() : (void *)out_rec.data(), is_sam, mrl};
   g_emu_leavable = true;
-  for (int t = 0; t < 3 && n_slots > 0; ++t) {
-    HostTier &tier = tiers[t];
-    tier_prepare_host(tier, n_slots, pair_list, t == 0);
-    const Scratch S = tier.view;
-    rs.tier_pairs[t] = n_slots;
-    if (t == 0) {
-      // the front end: [adapter trimming] + length filter + minimizers + table probes over staged read tiles (seed_front_kernel, a
-      // persistent grid: three CTAs here, so that every CTA walks several tiles through both stages of its double buffer)
-      if (P.trim) launch((n_slots + TB - 1) / TB, TB, 0, [&]() { prep_kernel(P, B, S); });
-      {
-        const int tiles = (n_slots + SF_TILE - 1) / SF_TILE;
-        launch(front_only ? 2 : std::min(tiles, 3), SF_NT, seed_front_smem_bytes(S.caps.maxmm) + 16, [&]() { if (K == 17 && W == 7) seed_front_kernel<true>(P, ix, B, S, &ctr, P.trim ? 1 : 0, 0, n_slots); else seed_front_kernel<false>(P, ix, B, S, &ctr, P.trim ? 1 : 0, 0, n_slots); });
+  // the front end: [adapter trimming] + length filter + minimizers + table probes over staged read tiles (seed_front_kernel, a
+  // persistent grid: three CTAs here, so that every CTA walks several tiles through both stages of its double buffer)
+  const Scratch S = lane_front(x, a, (u32)n, front_only ? 2 : 3);
+  // cross-check of its records against the oracle's minimizers and khash lookups (what the kernel must have written)
+  for (int slot = 0; slot < n; ++slot) {
+    if (S.pmeta[slot].status != ST_OK) continue;
+    for (int mate = 0; mate < (P.se ? 1 : 2); ++mate) {
+      const ReadMeta &z = S.rmeta[2 * slot + mate];
+      const char *rd = mate == 0 ? s1.data() + o1[slot] : s2.data() + o2[slot];
+      std::vector<uint64_t> mh(4096), mhit(4096);
+      const int nm = orc_minimizers(rd, (u32)z.len, 0, K, W, mh.data(), mhit.data(), 4096);
+      bool ok = z.n_mm == nm && z.mm_done == 1;
+      const size_t mb_ = mm_base(S, slot, mate);
+      const int ms = mm_stride(S);
+      for (int i = 0; ok && i < nm; ++i) {
+        uint64_t key = 0, val = 0;
+        const int found = orc_index_lookup(oix, mh[i], &key, &val);
+        const u32 kind = found ? ((key & 1) ? 1u : 2u) : 0u;
+        ok = S.mm_pos[mb_ + (size_t)i * ms] == (((u32)mhit[i] & 0x3FFFFFFFu) | (kind << 30)) && (!found || S.mm_val[mb_ + (size_t)i * ms] == val);
       }
-      // cross-check of its records against the oracle's minimizers and khash lookups (what the kernel must have written)
-      for (int slot = 0; slot < n_slots; ++slot) {
-        if (S.pmeta[slot].status != ST_OK) continue;
-        for (int mate = 0; mate < (P.se ? 1 : 2); ++mate) {
-          const ReadMeta &z = S.rmeta[2 * slot + mate];
-          const char *rd = mate == 0 ? s1.data() + o1[slot] : s2.data() + o2[slot];
-          std::vector<uint64_t> mh(4096), mhit(4096);
-          const int nm = orc_minimizers(rd, (u32)z.len, 0, K, W, mh.data(), mhit.data(), 4096);
-          bool ok = z.n_mm == nm && z.mm_done == 1;
-          const size_t mb_ = mm_base(S, slot, mate);
-          const int ms = mm_stride(S);
-          for (int i = 0; ok && i < nm; ++i) {
-            uint64_t key = 0, val = 0;
-            const int found = orc_index_lookup(oix, mh[i], &key, &val);
-            const u32 kind = found ? ((key & 1) ? 1u : 2u) : 0u;
-            ok = S.mm_pos[mb_ + (size_t)i * ms] == (((u32)mhit[i] & 0x3FFFFFFFu) | (kind << 30)) && (!found || S.mm_val[mb_ + (size_t)i * ms] == val);
-          }
-          if (!ok) { if (rs.bad < 8) printf("FRONT END pair %%d mate %%d: n_mm %%d / %%d\n", slot, mate, z.n_mm, nm); ++rs.bad; }
-        }
-      }
-      if (front_only) {   // (many tiles per CTA: both stages of the double buffer are refilled and both barrier phases flip)
-        rs.pairs = n_slots;
-        for (int slot = 0; slot < n_slots; ++slot) rs.records += S.rmeta[2 * slot].n_mm + S.rmeta[2 * slot + 1].n_mm;
-        g_emu_leavable = false;
-        orc_mapper_free(om); orc_index_free(oix); orc_reference_free(oref);
-        return rs;
-      }
-      std::vector<int> vlist((size_t)2 * n_slots + 8), rlist((size_t)n_slots + 8);
-      int d_count[4] = {0, 0, 0, 0};
-      int rows0 = (2 * mrl / (W + 1) + 15) / 16 * 16;
-      rows0 = std::max(16, std::min(rows0, S.caps.hc));
-      launch((2 * n_slots + CLUSTER_NT - 1) / CLUSTER_NT, CLUSTER_NT, (size_t)rows0 * CLUSTER_NT * 8, [&]() { cluster_kernel(P, ix, S, &ctr, 0, rows0, vlist.data(), &d_count[3]); });
-      if (rows0 < S.caps.hc)
-        launch((2 * n_slots + CLUSTER_NT - 1) / CLUSTER_NT, CLUSTER_NT, (size_t)S.caps.hc * CLUSTER_NT * 8, [&]() { cluster_kernel(P, ix, S, &ctr, 1, S.caps.hc, vlist.data(), &d_count[3]); });
-      launch((n_slots + TB - 1) / TB, TB, 0, [&]() { pair_candidates_kernel(P, ix, S, &ctr, 0, rlist.data(), &d_count[1]); });
-      launch((n_slots + 63) / 64, 64, 0, [&]() { pair_candidates_kernel(P, ix, S, &ctr, 1, rlist.data(), &d_count[1]); });
-      if (P.split) launch((2 * n_slots + TB - 1) / TB, TB, 0, [&]() { verify_split_kernel(P, R, B, S, &ctr); });
-      else {
-        launch((2 * n_slots + TB - 1) / TB, TB, 0, [&]() { verify_kernel(P, R, B, S, &ctr, 0, vlist.data(), &d_count[2]); });
-        launch((2 * n_slots + 63) / 64, 64, (size_t)2 * S.caps.maxmm * 64, [&]() { verify_kernel(P, R, B, S, &ctr, 1, vlist.data(), &d_count[2]); });
-      }
-      if (P.split) launch((n_slots + TB - 1) / TB, TB, 0, [&]() { pairing_split_kernel(P, S, nbest.data()); });
-      else launch((n_slots + TB - 1) / TB, TB, 0, [&]() { pairing_kernel(P, S, nbest.data()); });
-    } else {
-      auto cap_of = [](int c_) { int c = 1; while (c < c_) c <<= 1; return std::min(c, CTA_SORT_SMEM_MAX); };
-      const int c_seed = cap_of(2 * tier.caps.hc), c_pc = cap_of(tier.caps.hc), c_ver = cap_of(tier.caps.cc), c_pair = cap_of(tier.caps.mc);
-      launch((n_slots + TB - 1) / TB, TB, 0, [&]() { prep_kernel(P, B, S); });
-      launch(2 * n_slots, CTA_NT, (size_t)c_seed * 11 + (size_t)(tier.caps.maxmm + 1) * 12 + 16, [&]() { seed_cta_kernel(P, ix, B, S, tiers[0].view, &ctr, c_seed); });
-      const int lcap = std::min(tier.caps.cc, 512), fcap = 2 * tier.caps.cc;
-      const size_t pc_smem = pair_candidates_cta_smem(c_pc, lcap, tier.caps.maxmm, fcap);
-      const int pc_nt = pc_smem > 64 * 1024 ? PC_CTA_NT_MAX : CTA_NT;
-      launch(n_slots, pc_nt, pc_smem, [&]() { pair_candidates_cta_kernel(P, ix, S, &ctr, c_pc, lcap, fcap, nullptr, nullptr); });
-      if (P.split) launch(2 * n_slots, CTA_NT, (size_t)c_ver * 9, [&]() { verify_split_cta_kernel(P, R, B, S, &ctr, c_ver); });
-      else launch(2 * n_slots, tier.caps.cc > 1024 ? VERIFY_NT_MAX : CTA_NT, (size_t)c_ver * 9 + 2 * (size_t)tier.caps.maxmm + 16, [&]() { verify_cta_kernel(P, R, B, S, &ctr, c_ver); });
-      if (P.split) launch((n_slots + TB - 1) / TB, TB, 0, [&]() { pairing_split_kernel(P, S, nbest.data()); });
-      else launch(n_slots, CTA_NT, (size_t)c_pair * 10, [&]() { pairing_cta_kernel(P, S, nbest.data(), c_pair); });
-    }
-    std::vector<int> ovf((size_t)n_slots + 8);
-    int n_ovf = 0;
-    launch((n_slots + 255) / 256, 256, 0, [&]() { collect_overflow_kernel(S, ovf.data(), &n_ovf); });
-    tiers_used = t + 1;
-    if (n_ovf > 0 && t + 1 < 3) {
-      ovf.resize((size_t)n_ovf);
-      std::sort(ovf.begin(), ovf.end());
-      tiers[t + 1].list = ovf;
-      pair_list = tiers[t + 1].list.data();
-    } else if (n_ovf > 0) { printf("pairs left after the last tier: %%d\n", n_ovf); ++rs.bad; }
-    n_slots = n_ovf;
-  }
-  // one reference batch = all pairs here: taskloop chunks of n / (n / 5000) ...: a single chunk for n < 10000
-  int chunks[2] = {0, n};
-  launch(1, 128, 0, [&]() { select_kernel(P, 1, chunks, nbest.data(), sel.data(), mt_init); });
-  for (int t = tiers_used - 1; t >= 0; --t) {
-    const Scratch S = tiers[t].view;
-    if (mode == MODE_SAM_SE) launch((S.n_slots + TB - 1) / TB, TB, 0, [&]() { emit_sam_se_kernel(P, R, B, T, S, sel.data(), out_sam.data(), out_n.data(), &ctr); });
-    else if (mode == MODE_SAM) launch((S.n_slots + TB - 1) / TB, TB, 0, [&]() { emit_sam_kernel(P, R, B, T, S, sel.data(), out_sam.data(), out_n.data(), &ctr); });
-    else if (P.split) launch((S.n_slots + TB - 1) / TB, TB, 0, [&]() { emit_split_kernel(P, R, B, T, S, sel.data(), (OutPairs *)out_rec.data(), out_n.data(), &ctr); });
-    else if (P.se) launch((S.n_slots + TB - 1) / TB, TB, 0, [&]() { emit_se_kernel(P, R, B, T, S, sel.data(), out_rec.data(), out_n.data(), &ctr); });
-    else if (t > 0) launch(S.n_slots, CTA_NT, 0, [&]() { emit_cta_kernel(P, R, B, T, S, sel.data(), out_rec.data(), out_n.data(), &ctr); });
-    else {
-      std::vector<int4> emit_list((size_t)S.n_slots * max_best + 8);
-      int dp_count = 0;
-      launch((S.n_slots + TB - 1) / TB, TB, 0, [&]() { emit_kernel(P, R, B, T, S, sel.data(), out_rec.data(), out_n.data(), &ctr, emit_list.data(), &dp_count); });
-      launch((int)(((size_t)S.n_slots * max_best + TB - 1) / TB), TB, 0, [&]() { emit_dp_kernel(P, R, B, T, S, out_rec.data(), emit_list.data(), &dp_count); });
+      if (!ok) { if (rs.bad < 8) printf("FRONT END pair %%d mate %%d: n_mm %%d / %%d\n", slot, mate, z.n_mm, nm); ++rs.bad; }
     }
   }
+  if (front_only) {   // (many tiles per CTA: both stages of the double buffer are refilled and both barrier phases flip)
+    rs.pairs = n;
+    rs.tier_pairs[0] = n;
+    for (int slot = 0; slot < n; ++slot) rs.records += S.rmeta[2 * slot].n_mm + S.rmeta[2 * slot + 1].n_mm;
+    g_emu_leavable = false;
+    orc_mapper_free(om); orc_index_free(oix); orc_reference_free(oref);
+    return rs;
+  }
+  const LaneTiers tiers = lane_tiers(x, a, S);
+  for (int t = 0; t < tiers.used; ++t) rs.tier_pairs[t] = tiers.S[t].n_slots;
+  if (tiers.n_left > 0) { printf("pairs left after the last tier: %%d\n", tiers.n_left); ++rs.bad; }
+  lane_emit(x, a, tiers, (u32)n);   // all pairs one reference batch
   g_emu_leavable = false;
   // ---- compare, pair by pair
   if (is_sam) {
@@ -344,9 +292,9 @@ int main() {
   static_assert(sizeof(OutRecord) == sizeof(orc_pe_record) && sizeof(OutPairs) == sizeof(orc_pe_record), "record layouts");
   long bad = 0;
   const int mrl = 80;
-  const Caps real[3] = {{mrl, 64, 32, 32}, {mrl * 2, 1024, 256, 256}, {mrl * 4, 65536, 8192, 8192}};   // the library's tiers
+  const Caps real[3] = {tier_caps(mrl, 0), tier_caps(mrl, 1), tier_caps(mrl, 2)};   // the library's tiers
   const Caps small[3] = {{mrl, 6, 2, 2}, {mrl * 2, 40, 6, 6}, {mrl * 4, 65536, 8192, 8192}};            // most pairs through the CTA kernels, some to the last tier
-  const Caps real_long[3] = {{150, 64, 32, 32}, {300, 1024, 256, 256}, {600, 65536, 8192, 8192}};
+  const Caps real_long[3] = {tier_caps(150, 0), tier_caps(150, 1), tier_caps(150, 2)};
   const Caps small_long[3] = {{150, 6, 2, 2}, {300, 40, 6, 6}, {600, 65536, 8192, 8192}};
   struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; Knobs knobs = {}; };
   const Case cases[] = {
