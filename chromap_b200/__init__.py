@@ -5,7 +5,8 @@ Thin ctypes view of the C ABI in include/chromap_b200.h (chromap_b200/libchromap
 anywhere, but creating a Mapper without the CUDA library or without a GPU raises.
 """
 from .binding import (Mapper, Params, PE_RECORD, PAIRS_RECORD, PAIR_TRACE, SAM_RECORD, Timing, CmxError, lib_path, load_library,
-                      make_params, taskloop_chunks, format_sam, format_paf, exchange_finish, ExchangeStats)
+                      make_params, taskloop_chunks, format_sam, format_paf, exchange_finish, ExchangeStats, ReadRange,
+                      parse_read_format, apply_read_range)
 
 __all__ = ["format_sam", "format_paf", "Mapper", "Params", "PE_RECORD", "PAIRS_RECORD", "PAIR_TRACE", "SAM_RECORD", "Timing", "CmxError", "lib_path", "load_library",
-           "make_params", "taskloop_chunks", "exchange_finish", "ExchangeStats"]
+           "make_params", "taskloop_chunks", "exchange_finish", "ExchangeStats", "ReadRange", "parse_read_format", "apply_read_range"]

@@ -89,6 +89,42 @@ class Ingested(C.Structure):
     _fields_ = [("n_reads", C.c_uint32), ("seq", C.c_void_p), ("off", C.c_void_p), ("qual", C.c_void_p), ("min_len", C.c_uint32), ("max_len", C.c_uint32)]
 
 
+MAX_READ_RANGES = 8
+
+
+class ReadRange(C.Structure):
+    """cmx_read_range: the part of every read of one file that --read-format keeps."""
+    _fields_ = [("n", C.c_uint32), ("start", C.c_int32 * MAX_READ_RANGES), ("end", C.c_int32 * MAX_READ_RANGES), ("reverse", C.c_int32)]
+
+    def ranges(self):
+        return [(self.start[k], self.end[k]) for k in range(self.n)]
+
+
+def parse_read_format(fmt):
+    """--read-format text -> (r1, r2, bc) ReadRange (host only).  Raises CmxError for a format outside the grammar and for
+    ranges the GPU path refuses (not ascending and disjoint, -1 before the last range, more than 8 per file)."""
+    L = load_library()
+    r = [ReadRange() for _ in range(3)]
+    rc = L.cmx_parse_read_format(fmt.encode() if isinstance(fmt, str) else fmt, *[C.byref(x) for x in r])
+    if rc == -3:
+        raise CmxError("Unknown read format: %s" % fmt)
+    if rc != 0:
+        raise CmxError("read format %s: ranges the GPU path refuses (%d)" % (fmt, rc))
+    return tuple(r)
+
+
+def apply_read_range(read_range, seq, qual=None):
+    """The cut of one read (host only): (seq, qual) bytes after it.  Raises CmxError when an explicit end is at or past the
+    read's length or nothing is left."""
+    L = load_library()
+    s = C.create_string_buffer(bytes(seq), len(seq))
+    q = C.create_string_buffer(bytes(qual), len(qual)) if qual is not None else None
+    n = L.cmx_apply_read_range(C.byref(read_range), s, q, len(seq))
+    if n <= 0:
+        raise CmxError("read of length %d: %s" % (len(seq), "empty after the cut" if n == 0 else "shorter than a range's end (%d)" % n))
+    return s.raw[:n], (q.raw[:n] if q is not None else None)
+
+
 class Batch(C.Structure):
     _fields_ = [("n_pairs", C.c_uint32), ("seq1", C.c_void_p), ("off1", C.c_void_p), ("seq2", C.c_void_p),
                 ("off2", C.c_void_p), ("first_read_id", C.c_uint32), ("on_device", C.c_int32),
@@ -204,6 +240,9 @@ def load_library():
     L.cmx_exchange_finish.argtypes = [C.POINTER(Params), vp, vp, u64]
     L.cmx_fastq_cut.restype = u64; L.cmx_fastq_cut.argtypes = [vp, u64, u32, C.POINTER(u32)]
     L.cmx_ingest_fastq.argtypes = [vp, i32, vp, u64, i32, vp, C.POINTER(Ingested)]
+    L.cmx_parse_read_format.argtypes = [C.c_char_p, C.POINTER(ReadRange), C.POINTER(ReadRange), C.POINTER(ReadRange)]
+    L.cmx_apply_read_range.restype = i64; L.cmx_apply_read_range.argtypes = [C.POINTER(ReadRange), vp, vp, u32]
+    L.cmx_ingest_fastq_range.argtypes = [vp, i32, vp, u64, i32, vp, C.POINTER(ReadRange), C.POINTER(Ingested)]
     _lib = L
     return L
 
@@ -439,13 +478,17 @@ class Mapper:
         b = self.L.cmx_fastq_cut(a.ctypes.data, len(a), max_records, C.byref(n))
         return b, n.value
 
-    def ingest_fastq(self, slot, text, want_qual=False, want_names=False):
-        """FASTQ text (whole records) -> packed reads on the device.  Returns (Ingested, name_spans | None)."""
+    def ingest_fastq(self, slot, text, want_qual=False, want_names=False, read_range=None):
+        """FASTQ text (whole records) -> packed reads on the device, cut by read_range (a ReadRange) if given.
+        Returns (Ingested, name_spans | None)."""
         a = np.frombuffer(text, dtype=np.uint8) if not isinstance(text, np.ndarray) else text
         spans = np.zeros(2 * (len(a) // 8 + 1), dtype=np.uint32) if want_names else None
         g = Ingested()
-        self._check(self.L.cmx_ingest_fastq(self.h, slot, a.ctypes.data, len(a), 1 if want_qual else 0, spans.ctypes.data if want_names else None, C.byref(g)),
-                    "cmx_ingest_fastq")
+        args = (self.h, slot, a.ctypes.data, len(a), 1 if want_qual else 0, spans.ctypes.data if want_names else None)
+        if read_range is None:
+            self._check(self.L.cmx_ingest_fastq(*args, C.byref(g)), "cmx_ingest_fastq")
+        else:
+            self._check(self.L.cmx_ingest_fastq_range(*args, C.byref(read_range), C.byref(g)), "cmx_ingest_fastq_range")
         return g, (spans[:2 * g.n_reads].reshape(-1, 2) if want_names else None)
 
     def set_lanes(self, n):

@@ -31,6 +31,7 @@
 #include "sam_kernels.cuh"
 #include "ingest.cuh"
 #include "lane_pipeline.cuh"
+#include "host/read_range.h"
 
 static_assert(sizeof(OutRecord) == sizeof(cmx_pe_record), "record layout");
 static_assert(sizeof(cmx_pe_record) == 24, "record size");
@@ -69,7 +70,7 @@ struct Lane {
 
 #define CMX_INGEST_SLOTS 6
 struct IngestSlot {  // buffers of one cmx_ingest_fastq stream (text in, packed reads out)
-  DevBuf text, nl, seq_start, qual_start, len, off, seq, qual, spans, tmp, stats, count;
+  DevBuf text, nl, seq_start, qual_start, len, off, seq, qual, spans, tmp, stats, count, cut_stats;
   Stream stream;
 };
 
@@ -891,7 +892,20 @@ uint64_t cmx_fastq_cut(const char *text, uint64_t n_bytes, uint32_t max_records,
 }
 
 int cmx_ingest_fastq(cmx_ctx *ctx, int slot, const char *text, uint64_t n_bytes, int want_qual, uint32_t *name_spans, cmx_ingested *out) {
+  return cmx_ingest_fastq_range(ctx, slot, text, n_bytes, want_qual, name_spans, nullptr, out);
+}
+
+int cmx_ingest_fastq_range(cmx_ctx *ctx, int slot, const char *text, uint64_t n_bytes, int want_qual, uint32_t *name_spans, const cmx_read_range *range,
+                           cmx_ingested *out) {
   if (!ctx || !out || slot < 0 || slot >= CMX_INGEST_SLOTS || (!text && n_bytes)) return CMX_ERR_INVALID;
+  if (range && !cmxhost::ReadRangeRepresentable(*range)) return fail(ctx, CMX_ERR_INVALID, "cmx_ingest_fastq_range: a read range that is not representable");
+  const bool cut = range && !cmxhost::ReadRangeIsWhole(*range);
+  static_assert(CUT_MAX_RANGES == CMX_MAX_READ_RANGES, "range count");
+  CutRanges cr{};
+  if (cut) {
+    cr.n = range->n; cr.reverse = range->reverse;
+    for (u32 k = 0; k < range->n; ++k) { cr.start[k] = range->start[k]; cr.end[k] = range->end[k]; }
+  }
   memset(out, 0, sizeof(*out));
   if (n_bytes == 0) return CMX_OK;
   if (n_bytes >= 0xFFFFFFF0ull) return fail(ctx, CMX_ERR_INVALID, "cmx_ingest_fastq: chunk of 4 GiB or more");
@@ -924,6 +938,12 @@ int cmx_ingest_fastq(cmx_ctx *ctx, int slot, const char *text, uint64_t n_bytes,
   CU(cudaMemsetAsync((u32 *)g.len.p + n, 0, 4, st));
   ingest_record_kernel<<<(n + 255) / 256, 256, 0, st>>>((const char *)g.text.p, (const u32 *)g.nl.p, n, (u32 *)g.seq_start.p, (u32 *)g.qual_start.p, (u32 *)g.len.p,
                                                         name_spans ? (u32 *)g.spans.p : nullptr, (IngestStats *)g.stats.p);
+  CutStats hc = {0, 0, 0xFFFFFFFFu, 0};
+  if (cut) {
+    CU(ensure(g.cut_stats, sizeof(CutStats)));
+    CU(cudaMemcpyAsync(g.cut_stats.p, &hc, sizeof(hc), cudaMemcpyHostToDevice, st));
+    ingest_cut_len_kernel<<<(n + 255) / 256, 256, 0, st>>>((u32 *)g.len.p, n, cr, (CutStats *)g.cut_stats.p);
+  }
   cub::DeviceScan::ExclusiveSum(nullptr, tb, (const u32 *)g.len.p, (u32 *)g.off.p, (int)n + 1, st);
   CU(ensure(g.tmp, tb));
   CU(cub::DeviceScan::ExclusiveSum(g.tmp.p, tb, (const u32 *)g.len.p, (u32 *)g.off.p, (int)n + 1, st));
@@ -931,15 +951,26 @@ int cmx_ingest_fastq(cmx_ctx *ctx, int slot, const char *text, uint64_t n_bytes,
   // pack kernel has run, so the buffers are sized by the chunk and the quality copy is bounded by the quality line itself
   CU(ensure(g.seq, n_bytes + 64));
   if (want_qual) CU(ensure(g.qual, n_bytes + 64));
-  ingest_pack_kernel<<<(unsigned)(((u64)n * 32 + 255) / 256), 256, 0, st>>>((const char *)g.text.p, (const u32 *)g.seq_start.p, (const u32 *)g.qual_start.p,
-                                                                           (const u32 *)g.off.p, (const u32 *)g.nl.p, n, (char *)g.seq.p, want_qual ? (char *)g.qual.p : nullptr);
+  // (a cut is never longer than its read: the same sizes hold)
+  if (cut)
+    ingest_cut_pack_kernel<<<(unsigned)(((u64)n * 32 + 255) / 256), 256, 0, st>>>((const char *)g.text.p, (const u32 *)g.seq_start.p, (const u32 *)g.qual_start.p,
+                                                                                 (const u32 *)g.off.p, (const u32 *)g.nl.p, n, cr, (char *)g.seq.p,
+                                                                                 want_qual ? (char *)g.qual.p : nullptr);
+  else
+    ingest_pack_kernel<<<(unsigned)(((u64)n * 32 + 255) / 256), 256, 0, st>>>((const char *)g.text.p, (const u32 *)g.seq_start.p, (const u32 *)g.qual_start.p,
+                                                                             (const u32 *)g.off.p, (const u32 *)g.nl.p, n, (char *)g.seq.p, want_qual ? (char *)g.qual.p : nullptr);
   CU(cudaMemcpyAsync(&hs, g.stats.p, sizeof(hs), cudaMemcpyDeviceToHost, st));
+  if (cut) CU(cudaMemcpyAsync(&hc, g.cut_stats.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
   if (name_spans) CU(cudaMemcpyAsync(name_spans, g.spans.p, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   CU(cudaGetLastError());
   if (hs.bad_header || hs.bad_plus) return fail(ctx, CMX_ERR_INVALID, "cmx_ingest_fastq: not 4-line FASTQ (%u headers without '@', %u separator lines without '+')", hs.bad_header, hs.bad_plus);
   if (hs.empty_reads) return fail(ctx, CMX_ERR_INVALID, "cmx_ingest_fastq: %u empty reads (the reference skips them per file; use the host reader)", hs.empty_reads);
   if (hs.qual_mismatch) return fail(ctx, CMX_ERR_INVALID, "cmx_ingest_fastq: %u records whose quality and sequence lengths differ", hs.qual_mismatch);
+  if (cut && (hc.out_of_range || hc.empty))
+    return fail(ctx, CMX_ERR_READ_RANGE, "cmx_ingest_fastq_range: %u reads end before a range of the read format does, %u reads are empty after the cut", hc.out_of_range,
+                hc.empty);
+  if (cut) { hs.min_len = hc.min_len; hs.max_len = hc.max_len; }
   out->n_reads = n; out->seq = (const char *)g.seq.p; out->off = (const uint32_t *)g.off.p; out->qual = want_qual ? (const char *)g.qual.p : nullptr;
   out->min_len = n ? hs.min_len : 0; out->max_len = hs.max_len;
   return CMX_OK;

@@ -220,9 +220,20 @@ struct RawFile {
 
 static double g_t_fill = 0, g_t_ingest = 0;  // loader thread: reading + cutting, device-side parsing (summed over calls)
 
+// --read-format: the ranges of read 1, read 2 and the barcode (whole reads without the option), and the refusal of reads
+// the reference would cut in an undefined way (a read shorter than an explicit range end, nothing left after the cut)
+struct ReadFormat {
+  std::string text;
+  cmx_read_range r[3];  // read 1, read 2, barcode
+};
+static void DieReadRange(const ReadFormat &rf, const std::string &detail) {
+  Die("chromap-b200: --read-format " + rf.text + " does not fit the reads (" + detail + "); the reference's output is undefined for them");
+}
+
 // One batch through the device-side parser.  Returns false if a file is not plain 4-line FASTQ (the caller then uses the
 // host reader); dies on real input errors, like LoadBatch.
-static bool LoadBatchGpu(cmx_ctx *ctx, RawFile *f1, RawFile *f2, RawFile *fb, int parity, uint32_t max_pairs, Batch *b, bool keep_names, uint32_t bc_len) {
+static bool LoadBatchGpu(cmx_ctx *ctx, RawFile *f1, RawFile *f2, RawFile *fb, int parity, uint32_t max_pairs, Batch *b, bool keep_names, uint32_t bc_len,
+                         const ReadFormat &rf) {
   b->Clear();
   uint32_t n1 = 0, n2 = 0, nb = 0;
   uint64_t c1 = 0, c2 = 0, cb = 0;  // the files are read (and inflated) side by side
@@ -243,10 +254,15 @@ static bool LoadBatchGpu(cmx_ctx *ctx, RawFile *f1, RawFile *f2, RawFile *fb, in
   cmx_ingested g1{}, g2{}, gb{};
   std::vector<uint32_t> spans;
   if (keep_names) spans.resize(2 * (size_t)n1);
-  if (cmx_ingest_fastq(ctx, parity * 3 + 0, f1->buf.data(), c1, 0, keep_names ? spans.data() : nullptr, &g1)) return false;
-  if (f2 && cmx_ingest_fastq(ctx, parity * 3 + 1, f2->buf.data(), c2, 0, nullptr, &g2)) return false;
+  auto ingest = [&](int which, RawFile *f, uint64_t bytes, int want_qual, uint32_t *name_spans, cmx_ingested *g) {
+    const int rc = cmx_ingest_fastq_range(ctx, parity * 3 + which, f->buf.data(), bytes, want_qual, name_spans, &rf.r[which], g);
+    if (rc == CMX_ERR_READ_RANGE) DieReadRange(rf, cmx_last_error(ctx));
+    return rc == 0;
+  };
+  if (!ingest(0, f1, c1, 0, keep_names ? spans.data() : nullptr, &g1)) return false;
+  if (f2 && !ingest(1, f2, c2, 0, nullptr, &g2)) return false;
   if (fb) {
-    if (cmx_ingest_fastq(ctx, parity * 3 + 2, fb->buf.data(), cb, 1, nullptr, &gb)) return false;
+    if (!ingest(2, fb, cb, 1, nullptr, &gb)) return false;
     if (gb.min_len != bc_len || gb.max_len != bc_len) Die("ERROR: barcode lengths are not equal in the sample!");
   }
   if (keep_names) for (uint32_t i = 0; i < n1; ++i) b->names1.emplace_back(f1->buf.data() + spans[2 * i], spans[2 * i + 1]);
@@ -275,25 +291,38 @@ static uint64_t BarcodeSeed(const std::string &s) {
   return seed;
 }
 
-static uint32_t LoadBatch(SeqReader &r1, SeqReader &r2, uint32_t max_pairs, Batch *b, bool keep_names, SeqReader *rb = nullptr, uint32_t bc_len = 0,
-                          bool se = false, bool keep_sam = false) {
+// the cut of one read as loaded (sequence_batch.cc:35,51): reads the reference would cut in an undefined way are counted
+static void CutRead(const cmx_read_range &r, std::string *s, std::string *q, uint32_t *n_short, uint32_t *n_empty) {
+  const int64_t l = cmx_apply_read_range(&r, &(*s)[0], q->empty() ? nullptr : &(*q)[0], (uint32_t)s->size());
+  if (l < 0) ++*n_short;
+  else if (l == 0) ++*n_empty;
+  s->resize(l < 0 ? 0 : (size_t)l);
+  if (!q->empty()) q->resize(s->size());
+}
+
+static uint32_t LoadBatch(SeqReader &r1, SeqReader &r2, uint32_t max_pairs, Batch *b, bool keep_names, SeqReader *rb, uint32_t bc_len,
+                          bool se, bool keep_sam, const ReadFormat &rf) {
   std::string n, s, q;
+  uint32_t n_short = 0, n_empty = 0;
   b->Clear();
   while (b->n < max_pairs) {
     bool a = r1.Next(&n, &s, &q);
     while (a && s.empty()) a = r1.Next(&n, &s, &q);
+    if (a) CutRead(rf.r[0], &s, &q, &n_short, &n_empty);
     if (a) { b->s1 += s; b->o1.push_back((uint32_t)b->s1.size()); if (keep_names) b->names1.push_back(n); if (keep_sam) { q.resize(s.size(), 'I'); b->q1 += q; } }
     bool c = a;  // single-end: no second file
     if (!se) {
       c = r2.Next(&n, &s, &q);
       while (c && s.empty()) c = r2.Next(&n, &s, &q);
+      if (c) CutRead(rf.r[1], &s, &q, &n_short, &n_empty);
       if (c) { b->s2 += s; b->o2.push_back((uint32_t)b->s2.size()); if (keep_sam) { b->names2.push_back(n); q.resize(s.size(), 'I'); b->q2 += q; } }
     }
     bool d = c;
     if (rb) {
       d = rb->Next(&n, &s, &q);
       while (d && s.empty()) d = rb->Next(&n, &s, &q);
-      if (d) {
+      if (d) CutRead(rf.r[2], &s, &q, &n_short, &n_empty);
+      if (d && !n_short && !n_empty) {
         if (s.size() != bc_len) Die("ERROR: barcode lengths are not equal in the sample!");
         q.resize(bc_len, 'I');
         b->bc += s; b->bq += q;
@@ -304,6 +333,8 @@ static uint32_t LoadBatch(SeqReader &r1, SeqReader &r2, uint32_t max_pairs, Batc
     if (a != c || c != d) Die("Numbers of reads and barcodes don't match!");
     ++b->n;
   }
+  if (n_short || n_empty)
+    DieReadRange(rf, std::to_string(n_short) + " reads end before a range of the read format does, " + std::to_string(n_empty) + " reads are empty after the cut");
   return b->n;
 }
 
@@ -316,6 +347,7 @@ int main(int argc, char **argv) {
   bool cell_level_dedup = false;  // remove_pcr_duplicates_at_bulk_level == false (mapping_parameters.h:49; --preset atac clears it)
   double bc_prob = 0.9;
   bool build_index = false, bed = false, user_set_format = false;
+  ReadFormat rf;
   int k = 17, w = 7, threads = 1;
   (void)threads;
   for (int i = 1; i < argc; ++i)
@@ -330,7 +362,12 @@ int main(int argc, char **argv) {
     auto val = [&]() -> std::string { if (i + 1 >= argc) Die("Option " + a + " is missing an argument"); return argv[++i]; };
     if (a == "--preset") val();
     else if (a == "-i" || a == "--build-index") build_index = true;
-    else if (a == "-h" || a == "--help") { printf("chromap-b200: chromap's paired-end BED path on H100 GPUs (subset of chromap options; see DESIGN.md)\n"); return 0; }
+    else if (a == "-h" || a == "--help") {
+      printf("chromap-b200: chromap's paired-end BED path on H100 GPUs (subset of chromap options; see DESIGN.md)\n"
+             "  --read-format STR   parts of read 1, read 2 and the barcode to keep, as chromap: comma-separated r1|r2|bc:start:end[:+|-]\n"
+             "                      (0-based, inclusive, end -1 = the last base; ranges of one file ascending, '-' reverse-complements)\n");
+      return 0;
+    }
     else if (a == "-v" || a == "--version") { fprintf(stderr, "chromap-b200 0.1 (parity target: chromap 0.3.3-r521)\n"); return 0; }
     else if (a == "-r" || a == "--ref") ref_path = val();
     else if (a == "-x" || a == "--index") index_path = val();
@@ -361,6 +398,7 @@ int main(int argc, char **argv) {
     else if (a == "--output-mappings-not-in-whitelist") out_nw = 1;
     else if (a == "--skip-barcode-check") skip_bc_check = true;
     else if (a == "--host-reader") host_reader = true;  // parse FASTQ on the host (multi-line records, FASTA reads)
+    else if (a == "--read-format") rf.text = val();
     else if (a == "-n" || a == "--max-num-best-mappings") p.max_num_best_mappings = atoi(val().c_str());
     else if (a == "--drop-repetitive-reads") p.drop_repetitive_reads = atoi(val().c_str());
     else if (a == "--remove-pcr-duplicates-at-cell-level") cell_level_dedup = true;   // chromap_driver.cc:395-400: the level only
@@ -369,7 +407,7 @@ int main(int argc, char **argv) {
     else if (a == "--cache-size" || a == "--cache-update-param" || a == "--frip-est-params" || a == "--k-for-minhash" || a == "-A" || a == "--match-score" ||
              a == "-B" || a == "--mismatch-penalty" || a == "-O" || a == "--gap-open-penalties" || a == "-E" || a == "--gap-extension-penalties") val();
     else if (a == "--debug-cache" || a == "--turn-off-num-uniq-cache-slots") {}
-    else if (a == "--chr-order" || a == "--pairs-natural-chr-order" || a == "--read-format" || a == "--barcode-translate" || a == "--allocate-multi-mappings" ||
+    else if (a == "--chr-order" || a == "--pairs-natural-chr-order" || a == "--barcode-translate" || a == "--allocate-multi-mappings" ||
              a == "-p" || a == "--matrix-output-prefix")
       Die("chromap-b200: option " + a + " changes the output in ways that are not on the GPU path; use the reference chromap for it");
     else if (a == "--TagAlign") p.output_format = 2;  // same records as BED, TagAlign / PairedTagAlign text (chromap_driver.cc:417-418)
@@ -380,6 +418,11 @@ int main(int argc, char **argv) {
     else Die("Unknown option " + a);
   }
   (void)bed; (void)user_set_format;
+  const int rf_rc = cmx_parse_read_format(rf.text.c_str(), &rf.r[0], &rf.r[1], &rf.r[2]);  // chromap.cc:825-865
+  if (rf_rc == CMX_ERR_INVALID) Die("Unknown read format: " + rf.text + "\n");
+  if (rf_rc != CMX_OK)
+    Die("chromap-b200: --read-format " + rf.text + ": the ranges of one file must ascend without overlapping, only the last may end at -1, and there may be up to " +
+        std::to_string(CMX_MAX_READ_RANGES) + "; the reference runs such a format, but its in-place cut makes the result an artifact, so the GPU path refuses it");
   if (!(((p.output_format == 1 || p.output_format == 2 || p.output_format == 4) && !p.split_alignment) || (p.output_format == 5 && p.split_alignment)))
     Die("chromap-b200: supported outputs are BED / TagAlign (no split alignment) and Hi-C pairs (--split-alignment --pairs / --preset hic)");
   const bool tagalign = p.output_format == 2;
@@ -477,7 +520,13 @@ int main(int argc, char **argv) {
     SeqReader rb0;
     if (!rb0.Open(bc_path)) Die("Cannot find sequence file " + bc_path);
     std::string n, s, q;
+    uint32_t n_short = 0, n_empty = 0;
+    auto cut = [&]() {  // every barcode is cut before its length or its key is looked at (chromap.cc:370, 494)
+      CutRead(rf.r[2], &s, &q, &n_short, &n_empty);
+      if (n_short || n_empty) DieReadRange(rf, n_short ? "a barcode ends before a range of the read format does" : "a barcode is empty after the cut");
+    };
     if (!rb0.Next(&n, &s, &q)) Die("Empty barcode file");
+    cut();
     bc_len = (uint32_t)s.size();
     if (bc_len > 32) Die("ERROR: barcode length is greater than 32!");
     if (!wl_path.empty()) {
@@ -500,6 +549,7 @@ int main(int argc, char **argv) {
         ++in_batch; ++loaded;
         more = rb0.Next(&n, &s, &q);
         while (more && s.empty()) more = rb0.Next(&n, &s, &q);
+        if (more) cut();
         if (in_batch == (uint64_t)p.batch_size || !more) {
           if (!skip_bc_check && num_sample * 20 < in_batch) Die("Less than 5% barcodes can be found or corrected based on the barcode whitelist.");
           if (num_sample >= 20000000ull) break;
@@ -534,12 +584,12 @@ int main(int argc, char **argv) {
   const uint32_t call_pairs = (uint32_t)p.batch_size * 4u;
   auto load = [&](Batch *b, int par) {
     if (gpu_reader) {
-      if (!LoadBatchGpu(ctx, &g1, se ? nullptr : &g2, sc ? &gb : nullptr, par, call_pairs, b, pairs, bc_len))
+      if (!LoadBatchGpu(ctx, &g1, se ? nullptr : &g2, sc ? &gb : nullptr, par, call_pairs, b, pairs, bc_len, rf))
         Die(std::string("chromap-b200: the read files are not plain 4-line FASTQ (") + cmx_last_error(ctx) + "); rerun with --host-reader");
-    } else LoadBatch(r1, r2, (uint32_t)p.batch_size, b, pairs || sam || paf, sc ? &rb : nullptr, bc_len, se, sam || paf);
+    } else LoadBatch(r1, r2, (uint32_t)p.batch_size, b, pairs || sam || paf, sc ? &rb : nullptr, bc_len, se, sam || paf, rf);
   };
   open_all(gpu_reader);
-  if (gpu_reader && !LoadBatchGpu(ctx, &g1, se ? nullptr : &g2, sc ? &gb : nullptr, parity, call_pairs, &cur, pairs, bc_len)) {
+  if (gpu_reader && !LoadBatchGpu(ctx, &g1, se ? nullptr : &g2, sc ? &gb : nullptr, parity, call_pairs, &cur, pairs, bc_len, rf)) {
     fprintf(stderr, "Read files are not plain 4-line FASTQ (%s): using the host reader.\n", cmx_last_error(ctx));
     g1.Close(); g2.Close(); gb.Close();
     gpu_reader = false;

@@ -56,3 +56,76 @@ __global__ void ingest_pack_kernel(const char *text, const u32 *seq_start, const
     for (u32 i = lane; i < ql; i += 32) qual[o + i] = text[q + i];
   }
 }
+
+// --read-format (sequence_effective_range.h:80-118) on the same records: a length pass between ingest_record_kernel and the
+// offset scan, and a pack kernel in ingest_pack_kernel's place.
+#define CUT_MAX_RANGES 8
+struct CutRanges {  // cmx_read_range as the kernels take it: ranges ascending and disjoint, end == -1 in the last one only
+  u32 n;
+  int start[CUT_MAX_RANGES], end[CUT_MAX_RANGES];
+  int reverse;
+};
+struct CutStats {  // device-side summary of the cut
+  u32 out_of_range, empty, min_len, max_len;
+};
+
+// one thread per record: raw length -> cut length, in place.  A record whose read ends before an explicit range end gets
+// length 0 (nothing is packed for it) and is counted; so is a record with nothing left after the cut.
+__global__ void ingest_cut_len_kernel(u32 *len, u32 n_rec, CutRanges range, CutStats *st) {
+  const u32 r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rec) return;
+  const u32 l = len[r];
+  u32 c = 0;
+  bool over = false;
+#pragma unroll
+  for (u32 k = 0; k < CUT_MAX_RANGES; ++k) {  // unrolled: constant indices keep the ranges in registers
+    if (k >= range.n) break;
+    const u32 a = (u32)range.start[k];
+    if (range.end[k] == -1) c += l > a ? l - a : 0u;  // the last range only
+    else {
+      over |= (u32)range.end[k] >= l;
+      c += (u32)range.end[k] - a + 1u;
+    }
+  }
+  if (over) { atomicAdd(&st->out_of_range, 1u); c = 0; }
+  else if (c == 0) atomicAdd(&st->empty, 1u);
+  atomicMin(&st->min_len, c);
+  atomicMax(&st->max_len, c);
+  len[r] = c;
+}
+
+// ACGTacgt -> the upper-case complement, every other byte -> 'N' (utils.h:87-100)
+struct CutComplement {
+  u8 c[256];
+};
+constexpr CutComplement make_cut_complement() {
+  CutComplement t{};
+  for (int i = 0; i < 256; ++i) t.c[i] = 'N';
+  t.c['A'] = t.c['a'] = 'T'; t.c['C'] = t.c['c'] = 'G'; t.c['G'] = t.c['g'] = 'C'; t.c['T'] = t.c['t'] = 'A';
+  return t;
+}
+__device__ const CutComplement kCutComplement = make_cut_complement();
+
+// one warp per record: gather the bases (and qualities) of its ranges straight from the text to their packed place; with
+// range.reverse the bases are complemented and both are written back to front.  Reads and writes of a warp are consecutive
+// bytes either way.  The quality copy stays inside the quality line (see ingest_pack_kernel).
+__global__ void ingest_cut_pack_kernel(const char *text, const u32 *seq_start, const u32 *qual_start, const u32 *off, const u32 *nl, u32 n_rec,
+                                       CutRanges range, char *seq, char *qual) {
+  const u32 r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (r >= n_rec) return;
+  const u32 o = off[r], l = off[r + 1] - o, s = seq_start[r];
+  const u32 q = qual ? qual_start[r] : 0u, qe = qual ? nl[4 * r + 3] - q : 0u;
+  const bool rev = range.reverse != 0;
+  u32 done = 0;  // bases of the cut before range k
+  for (u32 k = 0; k < range.n && done < l; ++k) {
+    const u32 a = (u32)range.start[k];
+    const u32 m = range.end[k] == -1 ? l - done : min(l - done, (u32)range.end[k] - a + 1u);
+    for (u32 i = lane; i < m; i += 32) {
+      const u32 dst = o + (rev ? l - 1u - (done + i) : done + i);
+      const u8 b = (u8)text[s + a + i];
+      seq[dst] = rev ? (char)kCutComplement.c[b] : (char)b;
+      if (qual && a + i < qe) qual[dst] = text[q + a + i];
+    }
+    done += m;
+  }
+}

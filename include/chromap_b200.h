@@ -26,7 +26,8 @@ typedef enum {
   CMX_ERR_INVALID = -3,     /* bad argument / unsupported parameter combination */
   CMX_ERR_STATE = -4,       /* index or reference not uploaded yet */
   CMX_ERR_OVERFLOW = -5,    /* a pair exceeded even the large scratch tier (reported, never silent) */
-  CMX_ERR_IO = -6
+  CMX_ERR_IO = -6,
+  CMX_ERR_READ_RANGE = -7   /* --read-format ranges the reference cuts in an undefined way (see cmx_read_range) */
 } cmx_status;
 
 /* POD mirror of the MappingParameters fields the path reads (mapping_parameters.h:18-78). */
@@ -267,6 +268,36 @@ typedef struct {
 } cmx_ingested;
 uint64_t cmx_fastq_cut(const char *text, uint64_t n_bytes, uint32_t max_records, uint32_t *n_records);
 int cmx_ingest_fastq(cmx_ctx *ctx, int slot, const char *text, uint64_t n_bytes, int want_qual, uint32_t *name_spans, cmx_ingested *out);
+
+/* --read-format (chromap.cc:825-865, sequence_effective_range.h:20-118): the part of every read of one file that is kept.
+ * Ranges are 0-based and inclusive, concatenated in order; end == -1 is the read's last base.  reverse = 1 ('-' strand):
+ * after the cut the bases are complemented (ACGTacgt -> upper-case complement, any other byte -> N, utils.h:87-100) and
+ * reversed, the qualities reversed.  {1, {0}, {-1}, 0} keeps the whole read.
+ * Only cuts whose result the reference defines are representable: 1..CMX_MAX_READ_RANGES ranges, 0 <= start <= end,
+ * ascending and disjoint, -1 in the last range only (Replace copies in place: a range that reaches back would read bytes
+ * already overwritten). */
+#define CMX_MAX_READ_RANGES 8
+typedef struct {
+  uint32_t n;
+  int32_t start[CMX_MAX_READ_RANGES], end[CMX_MAX_READ_RANGES];
+  int32_t reverse;
+} cmx_read_range;
+/* Host only.  Parses "r1|r2|bc:start:end[:+|-]" fields separated by commas (start >= 0 and end >= start, or end == -1);
+ * fields of one file append ranges, the last strand given wins, a file named in no field keeps its whole read ("" = no
+ * cut at all).  CMX_ERR_INVALID for anything outside that grammar (the reference's hand parser accepts some such strings,
+ * with meanings that are artifacts of its loop); CMX_ERR_READ_RANGE for ranges of one file that are not representable
+ * above (the reference runs them, with an output that depends on its in-place copy). */
+int cmx_parse_read_format(const char *fmt, cmx_read_range *r1, cmx_read_range *r2, cmx_read_range *bc);
+/* Host only: the cut of one read in place (SequenceEffectiveRange::Replace); qual (may be NULL) gets the same ranges and
+ * order, not complemented.  Returns the new length; 0 if nothing is left (start >= len in the last, open-ended range);
+ * CMX_ERR_READ_RANGE if an explicit end is at or past len (the reference then reads past the string); CMX_ERR_INVALID for
+ * a range that is not representable. */
+int64_t cmx_apply_read_range(const cmx_read_range *range, char *seq, char *qual, uint32_t len);
+/* cmx_ingest_fastq with every record cut by `range` on the device (NULL or the whole read: exactly cmx_ingest_fastq).
+ * min_len / max_len are the cut lengths.  CMX_ERR_READ_RANGE, with the counts in cmx_last_error(), if a record is too short
+ * for an explicit end or empty after the cut. */
+int cmx_ingest_fastq_range(cmx_ctx *ctx, int slot, const char *text, uint64_t n_bytes, int want_qual, uint32_t *name_spans, const cmx_read_range *range,
+                           cmx_ingested *out);
 
 /* SAM text from the cores (host only, no device): expands them to one line per mate, puts them in SAMMapping's order,
  * removes duplicates / filters by MAPQ as the context's parameters say (sam_mapping.h:188-199, mapping_processor.h:161-202,
