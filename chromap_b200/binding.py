@@ -125,6 +125,67 @@ def apply_read_range(read_range, seq, qual=None):
     return s.raw[:n], (q.raw[:n] if q is not None else None)
 
 
+class _Translation(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("keys", C.c_void_p), ("to_off", C.c_void_p), ("to", C.c_void_p), ("from_len", C.c_uint32)]
+
+
+class BarcodeNotTranslated(CmxError):
+    """A barcode segment has no entry in the --barcode-translate table (CMX_ERR_BARCODE_TRANSLATE)."""
+
+
+class BarcodeTranslation:
+    """A --barcode-translate table: distinct FROM keys (2 bits per base), the TO string of each (bytes) and the FROM length L."""
+
+    def __init__(self, keys, to, from_len):
+        self.keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        self.to = [bytes(t) for t in to]
+        self.from_len = int(from_len)
+        assert len(self.keys) == len(self.to)
+        self._off = np.zeros(len(self.to) + 1, dtype=np.uint64)
+        self._off[1:] = np.cumsum([len(t) for t in self.to], dtype=np.uint64)
+        self._blob = C.create_string_buffer(b"".join(self.to), int(self._off[-1]) + 1)
+
+    def struct(self):
+        """The cmx_barcode_translation view (valid while this object lives)."""
+        return _Translation(len(self.keys), self.keys.ctypes.data, self._off.ctypes.data, C.addressof(self._blob), self.from_len)
+
+
+def parse_barcode_translation(data):
+    """Bytes of a --barcode-translate file (already inflated) -> BarcodeTranslation (host only).  Raises CmxError, naming the
+    line, for a table the GPU path refuses."""
+    L = load_library()
+    data = bytes(data)
+    t, err = _Translation(), C.create_string_buffer(256)
+    rc = L.cmx_parse_barcode_translation(data, len(data), C.byref(t), err, len(err))
+    if rc != 0:
+        raise CmxError("barcode translation table refused: " + err.value.decode())
+    try:
+        off = np.ctypeslib.as_array(C.cast(t.to_off, C.POINTER(C.c_uint64)), (t.n + 1,)).copy()
+        keys = np.ctypeslib.as_array(C.cast(t.keys, C.POINTER(C.c_uint64)), (t.n,)).copy()
+        blob = C.string_at(t.to, int(off[-1])) if off[-1] else b""
+        return BarcodeTranslation(keys, [blob[off[i]:off[i + 1]] for i in range(t.n)], t.from_len)
+    finally:
+        L.cmx_free_barcode_translation(C.byref(t))
+
+
+def format_bed_bc_tr(names, recs, bcs, bc_len, translation):
+    """Barcoded BED text on the host with a BarcodeTranslation applied (None: the untranslated text), the twin of
+    Mapper.format_bed_gpu with an uploaded table.  Raises BarcodeNotTranslated."""
+    L = load_library()
+    arr = (C.c_char_p * len(names))(*[s.encode() for s in names])
+    recs = np.ascontiguousarray(recs); bcs = np.ascontiguousarray(bcs, dtype=np.uint64)
+    t = translation.struct() if translation is not None else None
+    args = (arr, recs.ctypes.data, bcs.ctypes.data, len(recs), bc_len, C.byref(t) if t is not None else None)
+    n = L.cmx_format_bed_bc_tr(*args, None, 0)
+    if n == -8:
+        raise BarcodeNotTranslated("Barcode does not exist in the translation table.")
+    if n < 0:
+        raise CmxError("cmx_format_bed_bc_tr failed (%d)" % n)
+    buf = C.create_string_buffer(n + 1)
+    assert L.cmx_format_bed_bc_tr(*args, buf, n) == n
+    return buf.raw[:n]
+
+
 class Batch(C.Structure):
     _fields_ = [("n_pairs", C.c_uint32), ("seq1", C.c_void_p), ("off1", C.c_void_p), ("seq2", C.c_void_p),
                 ("off2", C.c_void_p), ("first_read_id", C.c_uint32), ("on_device", C.c_int32),
@@ -242,6 +303,10 @@ def load_library():
     L.cmx_ingest_fastq.argtypes = [vp, i32, vp, u64, i32, vp, C.POINTER(Ingested)]
     L.cmx_parse_read_format.argtypes = [C.c_char_p, C.POINTER(ReadRange), C.POINTER(ReadRange), C.POINTER(ReadRange)]
     L.cmx_apply_read_range.restype = i64; L.cmx_apply_read_range.argtypes = [C.POINTER(ReadRange), vp, vp, u32]
+    L.cmx_parse_barcode_translation.argtypes = [C.c_char_p, u64, C.POINTER(_Translation), vp, u64]
+    L.cmx_free_barcode_translation.restype = None; L.cmx_free_barcode_translation.argtypes = [C.POINTER(_Translation)]
+    L.cmx_upload_barcode_translation.argtypes = [vp, C.POINTER(_Translation)]
+    L.cmx_format_bed_bc_tr.restype = i64; L.cmx_format_bed_bc_tr.argtypes = [vp, vp, vp, u64, u32, C.POINTER(_Translation), vp, i64]
     L.cmx_ingest_fastq_range.argtypes = [vp, i32, vp, u64, i32, vp, C.POINTER(ReadRange), C.POINTER(Ingested)]
     _lib = L
     return L
@@ -363,6 +428,11 @@ class Mapper:
         keys = np.ascontiguousarray(keys, dtype=np.uint64); counts = np.ascontiguousarray(counts, dtype=np.uint32)
         self._check(self.L.cmx_upload_barcode_whitelist(self.h, keys.ctypes.data, counts.ctypes.data, len(keys), int(num_sample), bc_len,
                                                         err_threshold, prob_threshold, int(output_not_in_whitelist)), "cmx_upload_barcode_whitelist")
+
+    def upload_barcode_translation(self, translation):
+        """Put a BarcodeTranslation on the device (None removes it): format_bed_gpu then writes translated barcode fields."""
+        t = translation.struct() if translation is not None else None
+        self._check(self.L.cmx_upload_barcode_translation(self.h, C.byref(t) if t is not None else None), "cmx_upload_barcode_translation")
 
     def map_batch(self, seq1, off1, seq2, off2, first_read_id=0, on_device=False, n_pairs=None, out=None, out_on_device=False,
                   barcodes=None, barcode_quals=None, bc_len=0):
@@ -566,6 +636,9 @@ class Mapper:
         self.L.cmx_format_bed_bc(arr, recs.ctypes.data, bcs.ctypes.data, len(recs), bc_len, buf, n)
         return buf.raw[:n]
 
+    def format_bed_bc_tr(self, recs, bcs, bc_len, translation, names=None):
+        return format_bed_bc_tr(names or self.names, recs, bcs, bc_len, translation)
+
     def format_bed_gpu(self, recs, bcs=None, bc_len=0, names=None):
         """BED text written on the device; byte-identical to format_bed / format_bed_bc."""
         names = names or self.names
@@ -576,6 +649,8 @@ class Mapper:
             bcs = np.ascontiguousarray(bcs, dtype=np.uint64)
             bp = bcs.ctypes.data
         n = self.L.cmx_format_bed_gpu(self.h, arr, recs.ctypes.data, bp, len(recs), bc_len, None, 0)
+        if n == -8:
+            raise BarcodeNotTranslated(self.L.cmx_last_error(self.h).decode())
         if n < 0:
             raise RuntimeError("cmx_format_bed_gpu: " + self.L.cmx_last_error(self.h).decode())
         buf = C.create_string_buffer(n + 1)

@@ -101,6 +101,11 @@ struct cmx_ctx {
   int wl_err = 1, wl_output_nw = 0, wl_active = 0;
   double wl_prob = 0.9;
   DevBuf bc_seq, bc_qual;
+  // --barcode-translate table (cmx_upload_barcode_translation); tr_n_slots == 0: none
+  DevMem<ulonglong2> tr_slots;
+  DevMem<char> tr_to;
+  u64 tr_n_slots = 0;
+  u32 tr_from_len = 0;
   // mapq tables
   DevMem<double> inv_log;
   DevMem<int> pen_thr;
@@ -428,6 +433,42 @@ int cmx_upload_barcode_whitelist(cmx_ctx *ctx, const uint64_t *keys, const uint3
   }
   ctx->wl_slots = std::move(slots); ctx->wl_n_slots = ns; ctx->wl_num_sample = num_sample; ctx->wl_bc_len = bc_len; ctx->wl_err = err_threshold; ctx->wl_prob = prob_threshold;
   ctx->wl_output_nw = output_not_in_whitelist; ctx->wl_active = 1;
+  return CMX_OK;
+}
+
+int cmx_upload_barcode_translation(cmx_ctx *ctx, const cmx_barcode_translation *t) {
+  if (!ctx) return CMX_ERR_INVALID;
+  if (t && (t->from_len < 1 || t->from_len > 31 || (t->n && (!t->keys || !t->to_off || (!t->to && t->to_off[t->n])))))
+    return fail(ctx, CMX_ERR_INVALID, "barcode translation: FROM length %u (1..31) or missing arrays", t->from_len);
+  CU(cudaSetDevice(ctx->device));
+  // the old table goes before the new one is allocated; a failed upload leaves none
+  ctx->tr_slots.reset(); ctx->tr_to.reset(); ctx->tr_n_slots = 0; ctx->tr_from_len = 0;
+  if (!t) return CMX_OK;
+  const u64 n = t->n;
+  std::vector<u64> vals(n);
+  for (u64 i = 0; i < n; ++i) {
+    const u64 len = t->to_off[i + 1] - t->to_off[i];
+    if (t->to_off[i + 1] < t->to_off[i] || len > 0xFFFFu || t->to_off[i] >> 48) return fail(ctx, CMX_ERR_INVALID, "barcode translation: TO string %llu out of range", (unsigned long long)i);
+    vals[i] = t->to_off[i] << 16 | len;
+  }
+  u64 ns = 64;
+  while (ns < 2 * n) ns <<= 1;
+  DevMem<ulonglong2> slots;
+  DevMem<char> to;
+  CU(slots.alloc(ns * sizeof(ulonglong2)));
+  CU(cudaMemset(slots, 0xFF, ns * sizeof(ulonglong2)));
+  const u64 to_bytes = n ? t->to_off[n] : 0;
+  CU(to.alloc(to_bytes + 1));
+  if (to_bytes) CU(cudaMemcpy(to, t->to, to_bytes, cudaMemcpyHostToDevice));
+  if (n) {
+    DevMem<u64> dk, dv;
+    CU(dk.alloc(n * 8)); CU(dv.alloc(n * 8));
+    CU(cudaMemcpy(dk, t->keys, n * 8, cudaMemcpyHostToDevice)); CU(cudaMemcpy(dv, vals.data(), n * 8, cudaMemcpyHostToDevice));
+    tr_insert_kernel<<<(unsigned)((n + 255) / 256), 256>>>(dk, dv, n, slots, ns - 1, table_shift(ns));
+    CU(cudaGetLastError());
+    CU(cudaDeviceSynchronize());
+  }
+  ctx->tr_slots = std::move(slots); ctx->tr_to = std::move(to); ctx->tr_n_slots = ns; ctx->tr_from_len = t->from_len;
   return CMX_OK;
 }
 
@@ -1777,22 +1818,46 @@ static int format_bed_gpu(cmx_ctx *ctx, const char *const *names, const cmx_pe_r
   if (barcode_keys) CU(d_bc.alloc(nc * 8));
   cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_len.p, d_off.p, (int)nc + 1, st);
   CU(d_tmp.alloc(tmp_bytes));
-  for (u64 c0 = 0; c0 < n; c0 += CH) {
-    const u64 m = std::min(CH, n - c0);
-    const unsigned nb = (unsigned)((m + 255) / 256);
-    CU(cudaMemcpyAsync(d_rec, records + c0, m * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
-    if (barcode_keys) CU(cudaMemcpyAsync(d_bc, barcode_keys + c0, m * 8, cudaMemcpyHostToDevice, st));
-    CU(cudaMemsetAsync(d_len + m, 0, 4, st));
-    bed_len_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_noff, barcode_keys ? (int)bc_len : 0, d_len);
-    CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_len.p, d_off.p, (int)m + 1, st));
-    u64 bytes = 0;
-    CU(cudaMemcpyAsync(&bytes, d_off + m, 8, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
-    if (buf && *total + (int64_t)bytes <= cap) {
-      if (bytes > d_out.cap) CU(d_out.alloc(bytes + bytes / 8));  // (alloc frees the smaller buffer first)
-      bed_write_kernel<<<nb, 256, 0, st>>>(d_rec, d_bc, m, d_names, d_noff, barcode_keys ? (int)bc_len : 0, d_off, 0, d_out);
-      CU(cudaMemcpyAsync(buf + *total, d_out, bytes, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
+  // --barcode-translate: every segment must have an entry before any text is written.  The length pass counts those that do
+  // not; with more than one chunk, a first round of length passes checks the whole call before the round that writes.
+  BedTranslation T{};
+  DevMem<unsigned long long> d_miss;
+  const bool tr = barcode_keys && ctx->tr_n_slots;
+  if (tr) {
+    CU(d_miss.alloc(16));
+    const unsigned long long init[2] = {0ull, ~0ull};
+    CU(cudaMemcpyAsync(d_miss, init, 16, cudaMemcpyHostToDevice, st));
+    T.slots = ctx->tr_slots; T.mask = ctx->tr_n_slots - 1; T.shift = table_shift(ctx->tr_n_slots); T.from_len = (int)ctx->tr_from_len; T.to = ctx->tr_to;
+    T.n_missing = d_miss.p; T.first_missing = reinterpret_cast<unsigned *>(d_miss.p + 1);  // (a chunk has < 2^32 records)
+  }
+  for (int round = tr && buf && n > CH ? 0 : 1; round < 2; ++round) {
+    for (u64 c0 = 0; c0 < n; c0 += CH) {
+      const u64 m = std::min(CH, n - c0);
+      const unsigned nb = (unsigned)((m + 255) / 256);
+      CU(cudaMemcpyAsync(d_rec, records + c0, m * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
+      if (barcode_keys) CU(cudaMemcpyAsync(d_bc, barcode_keys + c0, m * 8, cudaMemcpyHostToDevice, st));
+      CU(cudaMemsetAsync(d_len + m, 0, 4, st));
+      bed_len_kernel<<<nb, 256, 0, st>>>(d_rec, m, d_noff, barcode_keys ? (int)bc_len : 0, d_len, d_bc, T);
+      CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_len.p, d_off.p, (int)m + 1, st));
+      u64 bytes = 0;
+      unsigned long long miss[2] = {0ull, 0ull};
+      CU(cudaMemcpyAsync(&bytes, d_off + m, 8, cudaMemcpyDeviceToHost, st));
+      if (tr) CU(cudaMemcpyAsync(miss, d_miss, 16, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      if (miss[0]) {  // the first chunk with a missing segment (the count covers the chunks so far, all of them without one)
+        const u64 first = c0 + (u32)miss[1];
+        std::string bc;
+        for (u32 j = 0; j < bc_len; ++j) bc += "ACGT"[(barcode_keys[first] >> ((bc_len - 1 - j) * 2)) & 3];
+        return fail(ctx, CMX_ERR_BARCODE_TRANSLATE, "%llu barcode segments have no entry in the translation table; the first is in barcode %s (record %llu)", miss[0],
+                    bc.c_str(), (unsigned long long)first);
+      }
+      if (round == 1 && buf && *total + (int64_t)bytes <= cap) {
+        if (bytes > d_out.cap) CU(d_out.alloc(bytes + bytes / 8));  // (alloc frees the smaller buffer first)
+        bed_write_kernel<<<nb, 256, 0, st>>>(d_rec, d_bc, m, d_names, d_noff, barcode_keys ? (int)bc_len : 0, d_off, 0, d_out, T);
+        CU(cudaMemcpyAsync(buf + *total, d_out, bytes, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
+      }
+      if (round == 1) *total += (int64_t)bytes;
     }
-    *total += (int64_t)bytes;
   }
   CU(cudaGetLastError());
   return CMX_OK;
@@ -1802,7 +1867,8 @@ int64_t cmx_format_bed_gpu(cmx_ctx *ctx, const char *const *names, const cmx_pe_
   if (!ctx || !names || (!records && n) || (barcode_keys && (bc_len == 0 || bc_len > 32))) return -1;
   if (cudaSetDevice(ctx->device) != cudaSuccess) return -1;
   int64_t total = 0;
-  return format_bed_gpu(ctx, names, records, barcode_keys, n, bc_len, buf, cap, &total) == CMX_OK ? total : -1;
+  const int rc = format_bed_gpu(ctx, names, records, barcode_keys, n, bc_len, buf, cap, &total);
+  return rc == CMX_OK ? total : rc == CMX_ERR_BARCODE_TRANSLATE ? rc : -1;
 }
 
 // Pairs text on the device (pairs_len_kernel / pairs_write_kernel), byte-identical to cmx_format_pairs: the header is

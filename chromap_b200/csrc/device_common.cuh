@@ -206,6 +206,27 @@ __device__ __forceinline__ int index_lookup(const DevIndex &ix, u64 mm_hash, u64
   }
 }
 
+// Keyed tables of the cell barcodes (the whitelist, the --barcode-translate table): 16-byte slots {key, value}, empty
+// key CMX_EMPTY_KEY, slot = fibonacci(key) >> shift, linear probing; mask = n_slots - 1.
+__device__ __forceinline__ bool kv_find(const ulonglong2 *slots, u64 mask, int shift, u64 key, u64 *val) {
+  u64 s = (key * 0x9E3779B97F4A7C15ull) >> shift;
+  for (;;) {
+    const ulonglong2 kv = __ldg(&slots[s]);
+    if (kv.x == CMX_EMPTY_KEY) return false;
+    if (kv.x == key) { *val = kv.y; return true; }
+    s = (s + 1) & mask;
+  }
+}
+// The slot that holds `key`, claimed for it if the key is new (concurrent inserts of other keys are safe).
+__device__ __forceinline__ ulonglong2 *kv_claim(ulonglong2 *slots, u64 mask, int shift, u64 key) {
+  u64 s = (key * 0x9E3779B97F4A7C15ull) >> shift;
+  for (;;) {
+    const u64 old = atomicCAS((unsigned long long *)&slots[s].x, (unsigned long long)CMX_EMPTY_KEY, (unsigned long long)key);
+    if (old == CMX_EMPTY_KEY || old == key) return &slots[s];
+    s = (s + 1) & mask;
+  }
+}
+
 // Bring the cache lines of [p, p + bytes) towards the SM ahead of a loop that reads them one byte at a time (the banded
 // aligners consume one reference base per column: without this every column waits for its own L2 round trip).
 __device__ __forceinline__ void prefetch_span(const void *p, int bytes) {

@@ -32,6 +32,28 @@ static void Die(const std::string &msg) {  // utils.h:71-74
   fprintf(stderr, "%s\n", msg.c_str());
   exit(255);
 }
+// --barcode-translate: the file's lines through zlib (plain or gzipped, as the reference's gzopen / gzgets), parsed before
+// any device work so that a table the GPU path refuses needs no device.  A file that cannot be opened has no lines.
+static bool LoadBarcodeTranslation(const std::string &path, cmx_barcode_translation *tr) {
+  std::string text;
+  gzFile f = gzopen(path.c_str(), "r");
+  if (f) {
+    char buf[1 << 16];
+    int got;
+    while ((got = gzread(f, buf, sizeof(buf))) > 0) text.append(buf, (size_t)got);
+    gzclose(f);
+  }
+  char err[256] = "";
+  if (cmx_parse_barcode_translation(text.data(), text.size(), tr, err, sizeof(err)) == CMX_OK) return true;
+  Die("chromap-b200: --barcode-translate " + path + ": " + (f ? std::string(err) : "cannot be read") +
+      "; the reference's result for such a table is undefined or an artifact of its reader, so the GPU path refuses it");
+  return false;
+}
+// Translate's failure (barcode_translator.h:87-91), without the partial output file the reference leaves behind
+static void DieBarcodeNotTranslated(const std::string &detail) {
+  fprintf(stderr, "Barcode does not exist in the translation table.\n");
+  Die("chromap-b200: " + detail + "; no output was written");
+}
 static double Now() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
 struct Batch {
@@ -341,7 +363,7 @@ static uint32_t LoadBatch(SeqReader &r1, SeqReader &r2, uint32_t max_pairs, Batc
 int main(int argc, char **argv) {
   cmx_params p;
   cmx_default_params(&p);
-  std::string preset, ref_path, index_path, r1_path, r2_path, out_path, bc_path, wl_path;
+  std::string preset, ref_path, index_path, r1_path, r2_path, out_path, bc_path, wl_path, tr_path;
   int bc_err = 1, out_nw = 0;
   bool skip_bc_check = false, host_reader = false, paf = false;
   bool cell_level_dedup = false;  // remove_pcr_duplicates_at_bulk_level == false (mapping_parameters.h:49; --preset atac clears it)
@@ -365,7 +387,9 @@ int main(int argc, char **argv) {
     else if (a == "-h" || a == "--help") {
       printf("chromap-b200: chromap's paired-end BED path on H100 GPUs (subset of chromap options; see DESIGN.md)\n"
              "  --read-format STR   parts of read 1, read 2 and the barcode to keep, as chromap: comma-separated r1|r2|bc:start:end[:+|-]\n"
-             "                      (0-based, inclusive, end -1 = the last base; ranges of one file ascending, '-' reverse-complements)\n");
+             "                      (0-based, inclusive, end -1 = the last base; ranges of one file ascending, '-' reverse-complements)\n"
+             "  --barcode-translate FILE  write barcoded BED fields through a TO,FROM (or TO<tab>FROM) table, plain or gzipped, as chromap\n"
+             "                      (e.g. ATAC to gene-expression barcodes of 10x Multiome); bulk runs ignore it\n");
       return 0;
     }
     else if (a == "-v" || a == "--version") { fprintf(stderr, "chromap-b200 0.1 (parity target: chromap 0.3.3-r521)\n"); return 0; }
@@ -396,6 +420,7 @@ int main(int argc, char **argv) {
     else if (a == "--bc-error-threshold") bc_err = atoi(val().c_str());
     else if (a == "--bc-probability-threshold") bc_prob = atof(val().c_str());
     else if (a == "--output-mappings-not-in-whitelist") out_nw = 1;
+    else if (a == "--barcode-translate") tr_path = val();
     else if (a == "--skip-barcode-check") skip_bc_check = true;
     else if (a == "--host-reader") host_reader = true;  // parse FASTQ on the host (multi-line records, FASTA reads)
     else if (a == "--read-format") rf.text = val();
@@ -407,7 +432,7 @@ int main(int argc, char **argv) {
     else if (a == "--cache-size" || a == "--cache-update-param" || a == "--frip-est-params" || a == "--k-for-minhash" || a == "-A" || a == "--match-score" ||
              a == "-B" || a == "--mismatch-penalty" || a == "-O" || a == "--gap-open-penalties" || a == "-E" || a == "--gap-extension-penalties") val();
     else if (a == "--debug-cache" || a == "--turn-off-num-uniq-cache-slots") {}
-    else if (a == "--chr-order" || a == "--pairs-natural-chr-order" || a == "--barcode-translate" || a == "--allocate-multi-mappings" ||
+    else if (a == "--chr-order" || a == "--pairs-natural-chr-order" || a == "--allocate-multi-mappings" ||
              a == "-p" || a == "--matrix-output-prefix")
       Die("chromap-b200: option " + a + " changes the output in ways that are not on the GPU path; use the reference chromap for it");
     else if (a == "--TagAlign") p.output_format = 2;  // same records as BED, TagAlign / PairedTagAlign text (chromap_driver.cc:417-418)
@@ -464,6 +489,8 @@ int main(int argc, char **argv) {
   if (!bc_path.empty() && p.remove_pcr_duplicates && p.low_memory_mode && !cell_level_dedup)  // mapping_writer.h:254-262: only the low-memory merge has the bulk-level variant
     Die("chromap-b200: bulk-level duplicate removal of barcoded data is not on the GPU path (use --preset atac or --remove-pcr-duplicates-at-cell-level)");
   if (out_path.empty()) Die("No output file specified!");
+  cmx_barcode_translation tr{};  // the writer loads the table in bulk runs too (mapping_writer.h:39-42), which then never use it
+  const bool translate = !tr_path.empty() && LoadBarcodeTranslation(tr_path, &tr);
   // start-up, three things at once (the reference does them one after the other, chromap.h:684-730): the reference sequences
   // are parsed by one thread, the index file is mapped and read ahead by the kernel, the CUDA context comes up on this thread
   Reference ref;
@@ -561,6 +588,7 @@ int main(int argc, char **argv) {
       for (const auto &kv : wl) { keys.push_back(kv.first); counts.push_back(kv.second); }
       if (cmx_upload_barcode_whitelist(ctx, keys.data(), counts.data(), keys.size(), num_sample, bc_len, bc_err, bc_prob, out_nw)) Die(cmx_last_error(ctx));
     }
+    if (translate && cmx_upload_barcode_translation(ctx, &tr)) Die(cmx_last_error(ctx));
   }
   // double-buffered batch loop: the loader thread prepares batch b+1 while the GPU maps batch b (chromap.h:871-877).
   // Reads are parsed on the device (cmx_ingest_fastq) when the files are plain 4-line FASTQ, else by the host reader.
@@ -722,7 +750,13 @@ int main(int argc, char **argv) {
     if (cmx_postprocess_gpu(ctx, all.data(), all_bc.data(), all.size(), &keep) && cmx_postprocess_bc(ctx, all.data(), all_bc.data(), all.size(), &keep)) Die(cmx_last_error(ctx));
     bytes = cmx_format_bed_gpu(ctx, names.data(), all.data(), all_bc.data(), keep, bc_len, nullptr, 0);  // text written on the device
     if (bytes >= 0) { text.resize((size_t)bytes + 1); bytes = cmx_format_bed_gpu(ctx, names.data(), all.data(), all_bc.data(), keep, bc_len, text.data(), bytes); }
-    if (bytes < 0) {
+    if (bytes == CMX_ERR_BARCODE_TRANSLATE) DieBarcodeNotTranslated(cmx_last_error(ctx));
+    if (bytes < 0 && translate) {
+      bytes = cmx_format_bed_bc_tr(names.data(), all.data(), all_bc.data(), keep, bc_len, &tr, nullptr, 0);
+      if (bytes == CMX_ERR_BARCODE_TRANSLATE) DieBarcodeNotTranslated("a barcode segment has no entry in the translation table");
+      text.resize((size_t)bytes + 1);
+      cmx_format_bed_bc_tr(names.data(), all.data(), all_bc.data(), keep, bc_len, &tr, text.data(), bytes);
+    } else if (bytes < 0) {
       bytes = cmx_format_bed_bc(names.data(), all.data(), all_bc.data(), keep, bc_len, nullptr, 0);
       text.resize((size_t)bytes + 1);
       cmx_format_bed_bc(names.data(), all.data(), all_bc.data(), keep, bc_len, text.data(), bytes);
@@ -751,5 +785,6 @@ int main(int argc, char **argv) {
   fprintf(stderr, "Sorted, deduped and outputed mappings in %.2fs.\nNumber of output mappings (passed filters): %llu\nTotal time: %.2fs.\n", Now() - t_pp,
           (unsigned long long)keep, Now() - t_start);
   cmx_destroy(ctx);
+  cmx_free_barcode_translation(&tr);
   return 0;
 }

@@ -2181,25 +2181,12 @@ struct DevWhitelist {
   int output_not_in_whitelist;
   int active;               // whitelist uploaded
 };
-__device__ __forceinline__ bool wl_find(const DevWhitelist &W, u64 key, u64 *count) {
-  u64 s = (key * 0x9E3779B97F4A7C15ull) >> W.shift;
-  for (;;) {
-    const ulonglong2 kv = __ldg(&W.slots[s]);
-    if (kv.x == CMX_EMPTY_KEY) return false;
-    if (kv.x == key) { *count = kv.y; return true; }
-    s = (s + 1) & W.mask;
-  }
-}
+__device__ __forceinline__ bool wl_find(const DevWhitelist &W, u64 key, u64 *count) { return kv_find(W.slots, W.mask, W.shift, key, count); }
 __global__ void wl_insert_kernel(const u64 *keys, const u32 *counts, u64 n, ulonglong2 *slots, u64 mask, int shift) {
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const u64 key = keys[i];
-  u64 s = (key * 0x9E3779B97F4A7C15ull) >> shift;
-  for (;;) {
-    const u64 old = atomicCAS((unsigned long long *)&slots[s].x, (unsigned long long)CMX_EMPTY_KEY, (unsigned long long)key);
-    if (old == CMX_EMPTY_KEY || old == key) { slots[s].y = counts[i]; return; }
-    s = (s + 1) & mask;
-  }
+  ulonglong2 *slot = kv_claim(slots, mask, shift, keys[i]);
+  slot->y = counts[i];
 }
 // utils.h:107-126: 2 bits per base, ambiguous base -> A
 __device__ __forceinline__ u64 barcode_seed(const u8 *s, int len) {

@@ -153,7 +153,46 @@ __device__ __forceinline__ char *put_dec(char *p, u32 v) {  // writes v, returns
   for (int i = d - 1; i >= 0; --i) { p[i] = (char)('0' + v % 10u); v /= 10u; }
   return p + d;
 }
-__global__ void bed_len_kernel(const PpRecord *recs, u64 n, const u32 *name_off, int bc_len, u32 *len) {
+// --barcode-translate on the device (cmx_upload_barcode_translation).  slots == nullptr: no table, the field is the barcode.
+struct BedTranslation {
+  const ulonglong2 *slots;  // {FROM key, TO offset << 16 | TO length}: kv_find's layout, as the whitelist's
+  u64 mask;                 // n_slots - 1
+  int shift;
+  int from_len;             // L, 1..31
+  const char *to;           // the TO strings
+  unsigned long long *n_missing;  // length pass: += segments without an entry
+  unsigned *first_missing;        // length pass: min over the launch's records i that have one
+};
+__global__ void tr_insert_kernel(const u64 *keys, const u64 *vals, u64 n, ulonglong2 *slots, u64 mask, int shift) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  ulonglong2 *slot = kv_claim(slots, mask, shift, keys[i]);
+  slot->y = vals[i];
+}
+// The barcode field of a barcoded line.  Without a table: the bc_len bases of the key (barcode_translator.h:114-123).  With
+// one (Translate, barcode_translator.h:72-101): the TO strings of the key's nseg = bc_len / L segments joined by '-',
+// segment s = the L bases that end (nseg - 1 - s) * L bases before the key's last, so the leading bc_len mod L bases play no
+// part and nseg == 0 gives an empty field.  Writes to p unless it is nullptr; returns the field's length and adds the
+// segments that have no entry to *n_missing (they contribute nothing).
+__device__ __forceinline__ u32 bed_barcode_field(const BedTranslation &T, u64 bc, int bc_len, char *p, u32 *n_missing) {
+  if (!T.slots) {
+    if (p) for (int j = 0; j < bc_len; ++j) p[j] = "ACGT"[(bc >> ((bc_len - 1 - j) * 2)) & 3];
+    return (u32)bc_len;
+  }
+  const int L = T.from_len, nseg = bc_len / L;
+  const u64 seg_mask = (1ull << (2 * L)) - 1;
+  u32 l = 0;
+  for (int s = 0; s < nseg; ++s) {
+    if (s) { if (p) p[l] = '-'; ++l; }
+    u64 v;
+    if (!kv_find(T.slots, T.mask, T.shift, (bc >> (2 * L * (nseg - 1 - s))) & seg_mask, &v)) { ++*n_missing; continue; }
+    const u32 tl = (u32)(v & 0xFFFFu);
+    if (p) { const char *t = T.to + (v >> 16); for (u32 k = 0; k < tl; ++k) p[l + k] = t[k]; }
+    l += tl;
+  }
+  return l;
+}
+__global__ void bed_len_kernel(const PpRecord *recs, u64 n, const u32 *name_off, int bc_len, u32 *len, const u64 *bcs = nullptr, BedTranslation T = {}) {
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const PpRecord r = recs[i];
@@ -161,12 +200,15 @@ __global__ void bed_len_kernel(const PpRecord *recs, u64 n, const u32 *name_off,
   const u32 nm = name_off[r.w[1] + 1] - name_off[r.w[1]];
   const u32 dups = (r.w[4] >> 8) & 0xFFu;
   u32 l = nm + 1 + dec_digits(start) + 1 + dec_digits(end) + 1;
-  if (bc_len > 0) l += (u32)bc_len + 1 + dec_digits(dups) + 1;
-  else l += 1 + 1 + dec_digits(pe_mapq(r)) + 1 + 1 + 1 + dec_digits(dups) + 1;
+  if (bc_len > 0) {
+    u32 n_missing = 0;
+    l += bed_barcode_field(T, T.slots ? bcs[i] : 0ull, bc_len, nullptr, &n_missing) + 1 + dec_digits(dups) + 1;
+    if (n_missing) { atomicAdd(T.n_missing, (unsigned long long)n_missing); atomicMin(T.first_missing, (unsigned)i); }
+  } else l += 1 + 1 + dec_digits(pe_mapq(r)) + 1 + 1 + 1 + dec_digits(dups) + 1;
   len[i] = l;
 }
 __global__ void bed_write_kernel(const PpRecord *recs, const u64 *bcs, u64 n, const char *names, const u32 *name_off, int bc_len,
-                                 const u64 *off, u64 base, char *out) {
+                                 const u64 *off, u64 base, char *out, BedTranslation T = {}) {
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const PpRecord r = recs[i];
@@ -178,8 +220,8 @@ __global__ void bed_write_kernel(const PpRecord *recs, const u64 *bcs, u64 n, co
   p = put_dec(p, r.w[2] + pe_len(r)); *p++ = '\t';
   const u32 dups = (r.w[4] >> 8) & 0xFFu;
   if (bc_len > 0) {
-    const u64 bc = bcs[i];
-    for (int j = 0; j < bc_len; ++j) *p++ = "ACGT"[(bc >> ((bc_len - 1 - j) * 2)) & 3];  // barcode_translator.h:114-123
+    u32 n_missing = 0;  // none: the length pass found every segment
+    p += bed_barcode_field(T, bcs[i], bc_len, p, &n_missing);
     *p++ = '\t';
   } else {
     *p++ = 'N'; *p++ = '\t';

@@ -27,7 +27,8 @@ typedef enum {
   CMX_ERR_STATE = -4,       /* index or reference not uploaded yet */
   CMX_ERR_OVERFLOW = -5,    /* a pair exceeded even the large scratch tier (reported, never silent) */
   CMX_ERR_IO = -6,
-  CMX_ERR_READ_RANGE = -7   /* --read-format ranges the reference cuts in an undefined way (see cmx_read_range) */
+  CMX_ERR_READ_RANGE = -7,  /* --read-format ranges the reference cuts in an undefined way (see cmx_read_range) */
+  CMX_ERR_BARCODE_TRANSLATE = -8 /* a barcode segment has no entry in the --barcode-translate table */
 } cmx_status;
 
 /* POD mirror of the MappingParameters fields the path reads (mapping_parameters.h:18-78). */
@@ -204,6 +205,37 @@ int64_t cmx_format_bed(const char *const *names, const cmx_pe_record *records, u
 int64_t cmx_format_tagalign(const char *const *names, const cmx_pe_record *records, uint64_t n, char *buf, int64_t cap);
 int64_t cmx_format_bed_gpu(cmx_ctx *ctx, const char *const *names, const cmx_pe_record *records, const uint64_t *barcode_keys,
                            uint64_t n, uint32_t bc_len, char *buf, int64_t cap);
+
+/* --barcode-translate (BarcodeTranslator, barcode_translator.h; loaded by the writer's constructor, mapping_writer.h:39-42):
+ * the barcode field of barcoded BED lines becomes the TO strings of the key's segments.  A table file has lines TO<sep>FROM,
+ * <sep> the first ',' or '\t'; the key of FROM is GenerateSeedFromSequence (utils.h:111-129).  With L the FROM length, a
+ * barcode of bc_len bases has nseg = bc_len / L segments, segment s being the L bases that end (nseg - 1 - s) * L bases
+ * before its last (the leading bc_len mod L bases are ignored); the field is their TO strings joined by '-', empty when
+ * nseg == 0.  Order and duplicate removal keep using the untranslated key. */
+typedef struct {
+  uint64_t n;        /* distinct FROM keys */
+  uint64_t *keys;    /* [n], in the order of their first line */
+  uint64_t *to_off;  /* [n + 1]: TO of keys[i] = to[to_off[i] .. to_off[i + 1]), from the key's last line */
+  char *to;          /* TO strings, concatenated (not NUL-terminated) */
+  uint32_t from_len; /* L, 1..31 */
+} cmx_barcode_translation;
+/* Host only.  text = the file's bytes (inflated), one table per file.  Refuses with CMX_ERR_INVALID, the reason and the
+ * 1-based line in err (err_cap bytes, may be NULL), what the reference reads in an undefined or accidental way: no line at
+ * all; an empty line, a line without a separator or with an empty FROM; a FROM byte outside ACGTacgt (N, the '\r' of CRLF);
+ * FROMs of different lengths; L >= 32; a line longer than 510 bytes before its newline (gzgets' 512-byte buffer splits it);
+ * a NUL byte.  A repeated FROM takes the TO of its last line; TO may be empty; the last line needs no newline.
+ * On success *out owns its arrays: release them with cmx_free_barcode_translation. */
+int cmx_parse_barcode_translation(const char *text, uint64_t n_bytes, cmx_barcode_translation *out, char *err, uint64_t err_cap);
+void cmx_free_barcode_translation(cmx_barcode_translation *t);
+/* The table on the device (HBM), replacing the previous one; NULL removes it.  While one is uploaded, cmx_format_bed_gpu with
+ * barcode_keys writes translated fields, and returns CMX_ERR_BARCODE_TRANSLATE before writing any text when a segment has no
+ * entry (where the reference prints "Barcode does not exist in the translation table." and exits 255, after part of the
+ * file); cmx_last_error() then gives the number of such segments and the first barcode, in output order, that has one. */
+int cmx_upload_barcode_translation(cmx_ctx *ctx, const cmx_barcode_translation *translation);
+/* Host twin of the translated text: cmx_format_bed_bc with `translation` applied (NULL: exactly cmx_format_bed_bc).  Returns
+ * the bytes (or the needed size if buf is NULL), CMX_ERR_BARCODE_TRANSLATE with nothing written if a segment has no entry. */
+int64_t cmx_format_bed_bc_tr(const char *const *names, const cmx_pe_record *records, const uint64_t *barcode_keys, uint64_t n, uint32_t bc_len,
+                             const cmx_barcode_translation *translation, char *buf, int64_t cap);
 /* Pairs text (header + lines of cmx_format_pairs) with the lines written on the device.  read_names[i] is the name of read
  * first_read_id + i (n_read_names of them). */
 int64_t cmx_format_pairs_gpu(cmx_ctx *ctx, const char *const *names, const uint32_t *lengths, uint32_t n_seq, const cmx_pairs_record *records,
