@@ -284,6 +284,7 @@ def load_library():
     L.cmx_stage_probe.argtypes = [vp, vp, u64, vp, vp, vp]
     L.cmx_stage_banded_align.argtypes = [vp, i32, i32, vp, vp, u64, vp, vp]
     L.cmx_stage_cta_sort.argtypes = [vp, vp, vp, u32, u32]
+    L.cmx_stage_correct_barcodes.argtypes = [vp, vp, vp, u64, u32, vp, vp, vp, vp]
     L.cmx_last_batch_trace.argtypes = [vp, vp, u32]
     L.cmx_last_batch_timing.argtypes = [vp, C.POINTER(Timing)]
     L.cmx_set_lanes.argtypes = [vp, i32]
@@ -699,6 +700,17 @@ class Mapper:
         tags = None if tags is None else np.ascontiguousarray(tags, dtype=np.uint8).copy()
         self._check(self.L.cmx_stage_cta_sort(self.h, keys.ctypes.data, None if tags is None else tags.ctypes.data, len(keys), sm_cap), "cmx_stage_cta_sort")
         return keys, tags
+
+    def stage_correct_barcodes(self, barcodes, quals, bc_len):
+        """CorrectBarcodeAt for n barcodes (uint8 arrays of n * bc_len ASCII bytes) against the uploaded whitelist, with the
+        kernels map_batch runs.  Returns (keys uint64[n], ok uint8[n], n_in_whitelist, n_corrected)."""
+        barcodes = np.ascontiguousarray(barcodes, dtype=np.uint8); quals = np.ascontiguousarray(quals, dtype=np.uint8)
+        n = barcodes.size // bc_len
+        keys = np.zeros(n, dtype=np.uint64); ok = np.zeros(n, dtype=np.uint8)
+        n_in, n_cor = C.c_uint64(), C.c_uint64()
+        self._check(self.L.cmx_stage_correct_barcodes(self.h, barcodes.ctypes.data, quals.ctypes.data, n, bc_len, keys.ctypes.data, ok.ctypes.data,
+                                                      C.byref(n_in), C.byref(n_cor)), "cmx_stage_correct_barcodes")
+        return keys, ok, n_in.value, n_cor.value
 
     def stage_banded_align(self, e, read_len, patterns, texts):
         patterns = np.ascontiguousarray(patterns, dtype=np.uint8); texts = np.ascontiguousarray(texts, dtype=np.uint8)

@@ -389,7 +389,9 @@ int main(int argc, char **argv) {
              "  --read-format STR   parts of read 1, read 2 and the barcode to keep, as chromap: comma-separated r1|r2|bc:start:end[:+|-]\n"
              "                      (0-based, inclusive, end -1 = the last base; ranges of one file ascending, '-' reverse-complements)\n"
              "  --barcode-translate FILE  write barcoded BED fields through a TO,FROM (or TO<tab>FROM) table, plain or gzipped, as chromap\n"
-             "                      (e.g. ATAC to gene-expression barcodes of 10x Multiome); bulk runs ignore it\n");
+             "                      (e.g. ATAC to gene-expression barcodes of 10x Multiome); bulk runs ignore it\n"
+             "  --bc-error-threshold INT  max Hamming distance allowed to correct a barcode against the whitelist: 0, 1 or 2 [1]\n"
+             "  --bc-probability-threshold FLT  min probability of the best correction among the candidates [0.9]\n");
       return 0;
     }
     else if (a == "-v" || a == "--version") { fprintf(stderr, "chromap-b200 0.1 (parity target: chromap 0.3.3-r521)\n"); return 0; }
@@ -443,6 +445,9 @@ int main(int argc, char **argv) {
     else Die("Unknown option " + a);
   }
   (void)bed; (void)user_set_format;
+  if (!bc_path.empty() && !wl_path.empty() && (bc_err < 0 || bc_err > 2))  // only a whitelist run corrects barcodes (chromap.h:897-909)
+    Die("chromap-b200: --bc-error-threshold " + std::to_string(bc_err) + ": use 0, 1 or 2. A barcode is corrected by at most two substitutions; at " +
+        "3 or more the reference lets that many Ns through but keeps the rest in the key as A, so the GPU path refuses it");
   const int rf_rc = cmx_parse_read_format(rf.text.c_str(), &rf.r[0], &rf.r[1], &rf.r[2]);  // chromap.cc:825-865
   if (rf_rc == CMX_ERR_INVALID) Die("Unknown read format: " + rf.text + "\n");
   if (rf_rc != CMX_OK)

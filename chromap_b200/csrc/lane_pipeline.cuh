@@ -81,6 +81,17 @@ struct LaneTiers {
 
 static const int LANE_TB = 128;
 
+// The barcode gate of n barcodes: keys, accept flags and the two counters.  At --bc-error-threshold 2 the barcodes that need a
+// search are corrected by barcode_correct2_kernel: first with hit lists in shared memory, then the few with more hits than
+// those hold, with a slab per warp.  ctr's list counters start at zero.
+template <class X>
+void lane_barcodes(X &x, const DevWhitelist &W, const u8 *bc_seq, const u8 *bc_qual, int bc_len, int n, u64 *bc_key, u8 *bc_ok, Counters *ctr) {
+  x(barcode_kernel, (n + 127) / 128, 128, 0, W, bc_seq, bc_qual, bc_len, n, bc_key, bc_ok, ctr);
+  if (!W.active || W.err_threshold != 2) return;
+  x(barcode_correct2_kernel, std::min((n + BC2_WARPS - 1) / BC2_WARPS, BC2_GRID_MAX), BC2_WARPS * 32, 0, W, bc_seq, bc_qual, bc_len, bc_key, bc_ok, ctr, 0);
+  x(barcode_correct2_kernel, BC2_SLAB_WARPS / BC2_WARPS, BC2_WARPS * 32, 0, W, bc_seq, bc_qual, bc_len, bc_key, bc_ok, ctr, 1);
+}
+
 // Tier 0 for all pairs, and its front end: [adapter trimming] + length filter + minimizers + index probe in one kernel over
 // staged read tiles (seed_front.cuh).  When the reads arrive in pieces of `piece` pairs, one grid per piece starts as soon
 // as the piece has landed; the rest of the upload hides behind it.  grid_cap: seed_front_kernel's persistent grid.

@@ -87,7 +87,9 @@ int cmx_index_info(const cmx_ctx *ctx, int *k, int *w, uint64_t *n_keys, uint64_
 /* scATAC barcode whitelist with the abundances of ComputeBarcodeAbundance (chromap.cc:388-548, a host pre-pass over the
  * barcode file): n distinct 2-bit packed keys (GenerateSeedFromSequence, utils.h:107-126), their counts among the
  * sampled barcodes and the sample size.  Enables CorrectBarcodeAt (chromap.cc:572-799) inside cmx_map_batch_pe.
- * err_threshold = --bc-error-threshold (0 or 1 on the GPU path), prob_threshold = --bc-probability-threshold. */
+ * err_threshold = --bc-error-threshold: 0, 1 or 2 substitutions (at 2 a barcode may carry up to two Ns); any other value
+ * returns CMX_ERR_INVALID, since the reference would leave the Ns beyond the second in the key as A.
+ * prob_threshold = --bc-probability-threshold. */
 int cmx_upload_barcode_whitelist(cmx_ctx *ctx, const uint64_t *keys, const uint32_t *counts, uint64_t n, uint64_t num_sample,
                                  uint32_t bc_len, int err_threshold, double prob_threshold, int output_not_in_whitelist);
 
@@ -257,6 +259,11 @@ int cmx_stage_banded_align(cmx_ctx *ctx, int e, int read_len, const char *patter
 /* The overflow tiers' CTA-cooperative bitonic sort on n keys (tags != NULL: (count desc, position asc) candidate
  * order, mapping_metadata.h:65-68 / candidate.h:23-33); sm_cap = shared-memory tile (power of two <= 4096). */
 int cmx_stage_cta_sort(cmx_ctx *ctx, uint64_t *keys, uint8_t *tags, uint32_t n, uint32_t sm_cap);
+/* CorrectBarcodeAt (chromap.cc:572-799) for n host barcodes of bc_len bases (ASCII bases and qualities, n*bc_len bytes each)
+ * against the uploaded whitelist, with the kernels cmx_map_batch_pe runs: out_key[i] = the 2-bit key afterwards, out_ok[i] =
+ * 1 if it is in the whitelist or corrected (or --output-mappings-not-in-whitelist), and the two counters of the batch. */
+int cmx_stage_correct_barcodes(cmx_ctx *ctx, const char *bc_seq, const char *bc_qual, uint64_t n, uint32_t bc_len,
+                               uint64_t *out_key, uint8_t *out_ok, uint64_t *n_in_whitelist, uint64_t *n_corrected);
 /* Per-pair counters after a full cmx_map_batch_pe (same fields as the oracle's trace). */
 typedef struct {
   int32_t n_minimizers[2];
