@@ -306,18 +306,14 @@ int cmx_upload_reference(cmx_ctx *ctx, uint32_t n_seq, const uint64_t *offsets, 
   // the old reference goes before the new one is allocated; a failed upload leaves none
   ctx->ref_seq.reset(); ctx->ref_off.reset(); ctx->ref_len.reset();
   ctx->n_seq = 0; ctx->h_ref_off.clear(); ctx->h_ref_len.clear();
-  // device layout: [64 NUL][seq0][64.. NUL][seq1]...  every sequence start 64-byte aligned, >= 64 NULs after each
-  const u64 PAD = 64;
   std::vector<u64> doff(n_seq);
   std::vector<u32> dlen(n_seq);
-  u64 cur = PAD;
   for (u32 i = 0; i < n_seq; ++i) {
     const u64 len = offsets[i + 1] - offsets[i];
     if (len >= 0xFFFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "reference sequence %u too long for 32-bit positions", i);
-    doff[i] = cur; dlen[i] = (u32)len;
-    cur = (cur + len + PAD + 63) / 64 * 64;
+    dlen[i] = (u32)len;
   }
-  const u64 ref_bytes = cur + PAD;
+  const u64 ref_bytes = ref_layout(n_seq, (const u64 *)offsets, doff.data());
   DevMem<u8> seq;
   DevMem<u64> d_off;
   DevMem<u32> d_len;

@@ -65,6 +65,20 @@ struct DevRef {
   u32 n_seq;
 };
 
+// Where cmx_upload_reference puts n_seq sequences (lengths offsets[i + 1] - offsets[i]) in DevRef::seq: REF_PAD NUL bytes,
+// then every sequence at a 64-byte aligned offset off[i] and followed by at least REF_PAD NUL bytes.  The aligners read up
+// to e bytes past a sequence's end (BandedTraceback, the split aligner's drop-off): the padding is what they find there.
+// Returns the size of the whole layout.
+#define REF_PAD 64
+inline u64 ref_layout(u32 n_seq, const u64 *offsets, u64 *off) {
+  u64 cur = REF_PAD;
+  for (u32 i = 0; i < n_seq; ++i) {
+    off[i] = cur;
+    cur = (cur + (offsets[i + 1] - offsets[i]) + REF_PAD + 63) / 64 * 64;
+  }
+  return cur + REF_PAD;
+}
+
 struct DevBatch {
   const u8 *seq1;
   const u32 *off1;

@@ -80,17 +80,24 @@ struct EmuLane {
 static char comp(char c) { switch (c) { case 'A': case 'a': return 'T'; case 'C': case 'c': return 'G'; case 'G': case 'g': return 'C'; case 'T': case 't': return 'A'; default: return 'N'; } }
 static std::string revc(const std::string &s) { std::string r(s.rbegin(), s.rend()); for (auto &c : r) c = comp(c); return r; }
 
-struct RunStats { long pairs = 0, records = 0, tier_pairs[3] = {0, 0, 0}, bad = 0; };
+struct RunStats {
+  long pairs = 0, records = 0, tier_pairs[3] = {0, 0, 0}, bad = 0;
+  // oracle records at the ends of reference sequences (runs with `edges`): starting within L + e of the start of a rid > 0, ending
+  // within e + 1 of a sequence's end, on a sequence shorter than 2L; and pairs whose mate-guided lookup ran with a window that begins
+  // below the start of a rid > 0 (`lookup_at_start`: a mate without candidates of its own mapped by the lookup, the whole fragment
+  // within 2 * max_insert of the rid's start, so the partner's candidate lies there too)
+  long edge_start = 0, edge_end = 0, short_seq = 0, lookup_at_start = 0;
+};
 
 enum { MODE_CHIP = 0, MODE_ATAC = 1, MODE_HIC = 2, MODE_SE = 3, MODE_SAM = 4, MODE_SAM_SE = 5 };
 // mapping knobs over the preset (-1: the preset's value): -e, -s, -f f0,f1, --drop-repetitive-reads, --min-read-length
 struct Knobs { int e = -1, min_seeds = -1, f0 = -1, f1 = -1, drop_rep = -1, min_read_len = -1; };
 static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *caps3, int max_best, int read_len_base, bool front_only = false, int K = 17, int W = 7, int fam_copies = 90,
-                         const Knobs &kn = Knobs{}) {
+                         const Knobs &kn = Knobs{}, bool edges = false) {
   std::mt19937 g((unsigned)seed);
   RunStats rs;
   // ---- reference: two sequences, a 300 bp family with many copies, a 2 kb segmental repeat, an N run
-  std::string seq[2] = {std::string(fam_copies > 200 ? 260000 : 70000, 'A'), std::string(fam_copies > 200 ? 200000 : 50000, 'A')};
+  std::vector<std::string> seq = {std::string(edges ? 50000 : fam_copies > 200 ? 260000 : 70000, 'A'), std::string(edges ? 20000 : fam_copies > 200 ? 200000 : 50000, 'A')};
   for (auto &s : seq) for (auto &c : s) c = "ACGT"[g() %% 4];
   std::string fam(300, 'A'); for (auto &c : fam) c = "ACGT"[g() %% 4];
   for (int q = 0; q < fam_copies; ++q) { std::string f2 = fam; for (int x = 0; x < (int)(g() %% 4); ++x) f2[g() %% 300] = "ACGT"[g() %% 4]; std::string &s = seq[g() %% 2]; s.replace(500 + g() %% (s.size() - 1500), 300, f2); }
@@ -98,10 +105,25 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   for (int q = 0; q < 12; ++q) { std::string &s = seq[g() %% 2]; s.replace(1000 + g() %% (s.size() - 4000), 2000, seg); }
   seq[0].replace(30000, 80, std::string(80, 'N'));
   for (int q = 0; q < 3000; ++q) { std::string &s = seq[g() %% 2]; const size_t at = g() %% s.size(); s[at] = (char)tolower(s[at]); }
-  std::string concat = seq[0] + seq[1];
-  const uint64_t offs[3] = {0, seq[0].size(), seq[0].size() + seq[1].size()};
-  const char *names[2] = {"chrA", "chrB"};
-  orc_reference *oref = orc_reference_from_memory(2, concat.data(), offs, names);
+  if (edges) {   // then many short sequences, as in a scaffold-level assembly: shorter than k + w - 1 (no minimizer), around L + 2e
+                 // (no valid candidate), around a fragment, and a spread up to 3 kbp
+    for (int len : {20, 30, 45, 60, 76, 80, 85, 90, 99, 100, 101, 110, 120, 136, 150, 180, 250, 400, 700, 1200, 3000}) seq.emplace_back((size_t)len, 'A');
+    for (int q = 0; q < 24; ++q) seq.emplace_back((size_t)(64 + 64 * (g() %% 46)), 'A');
+    for (size_t i = 2; i < seq.size(); ++i) {
+      for (auto &c : seq[i]) c = "ACGT"[g() %% 4];
+      // copies of the repeat family at both ends of the longer ones: with -f low enough a mate inside a copy has no candidates of
+      // its own and is found by the mate-guided lookup around its partner, near the sequence's start or end
+      if (seq[i].size() >= 1000) { seq[i].replace(0, 300, fam); seq[i].replace(seq[i].size() - 300, 300, fam); }
+    }
+  }
+  const u32 n_seq = (u32)seq.size();
+  std::string concat;
+  std::vector<u64> offs{0};
+  std::vector<std::string> nm;
+  std::vector<const char *> names;
+  for (u32 q = 0; q < n_seq; ++q) { concat += seq[q]; offs.push_back(concat.size()); nm.push_back("seq" + std::to_string(q)); }
+  for (auto &s : nm) names.push_back(s.c_str());
+  orc_reference *oref = orc_reference_from_memory(n_seq, concat.data(), (const uint64_t *)offs.data(), names.data());
   orc_index *oix = orc_index_build(oref, K, W);
   // ---- reads
   std::string s1, s2;
@@ -111,10 +133,21 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
     int L1 = read_len_base + (int)(g() %% 11) - 5, L2 = read_len_base + (int)(g() %% 11) - 5;
     if (kind == 0) L1 = mrl + 5 + (int)(g() %% 40);                   // longer than the first tier allows
     if (kind == 1) L2 = 20;                                           // below the length filter
-    const std::string &rsq = seq[g() %% 2];
-    const int frag = std::max(L1, L2) + (int)(g() %% 350);
-    size_t at = 200 + g() %% (rsq.size() - frag - 400);
+    const std::string &rsq = seq[g() %% (edges ? n_seq : 2)];
+    int frag = std::max(L1, L2) + (int)(g() %% 350);
+    size_t at;
+    if (!edges) at = 200 + g() %% (rsq.size() - frag - 400);
+    else {   // a third start within 40 bp of the sequence's start, a third end within 40 bp of its end, a third anywhere
+      const int longest = std::max(L1, L2), size = (int)rsq.size();
+      if (frag > size) frag = size > longest ? longest + (int)(g() %% (unsigned)(size - longest + 1)) : size;
+      const size_t room = rsq.size() - (size_t)frag, near = std::min<size_t>(room, 40) + 1;
+      const int where = (int)(g() %% 3);
+      const size_t d = g() %% (1 + g() %% near);   // (more often the nearer)
+      at = where == 0 ? d : where == 1 ? room - d : g() %% (room + 1);
+    }
     std::string F = rsq.substr(at, (size_t)frag);
+    while ((int)F.size() < std::max(L1, L2)) F += "ACGT"[g() %% 4];   // a sequence shorter than the reads: they run off its end
+    frag = (int)F.size();
     if (kind == 2 || (fam_copies > 200 && kind %% 2 == 0)) { F = fam + std::string(rsq, at, (size_t)std::max(0, frag - 300)); F.resize((size_t)frag, 'A'); }   // inside the repeat family
     if (kind == 3) for (auto &c : F) c = "ACGT"[g() %% 4];                                                             // junk
     std::string a = F.substr(0, (size_t)L1), b = revc(F.substr((size_t)(frag - L2), (size_t)L2));
@@ -162,8 +195,38 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   std::vector<orc_sam_record> want_sam;
   long n_want_sam = 0;
   if (is_sam) { want_sam.resize((size_t)n * max_best + 8); n_want_sam = (long)orc_map_sam_cores(om, (u32)n, s1.data(), o1.data(), is_se ? nullptr : s2.data(), is_se ? nullptr : o2.data(), first_read_id, want_sam.data(), (long)want_sam.size()); }
+  std::vector<orc_pair_trace> trace((size_t)n);
   const long n_want = is_sam ? 0 : mode == MODE_SE ? (long)orc_map_reads_se(om, (u32)n, s1.data(), o1.data(), first_read_id, want.data(), (long)want.size(), 1)
-                                      : (long)orc_map_pairs(om, (u32)n, s1.data(), o1.data(), s2.data(), o2.data(), first_read_id, want.data(), (long)want.size(), nullptr);
+                                      : (long)orc_map_pairs(om, (u32)n, s1.data(), o1.data(), s2.data(), o2.data(), first_read_id, want.data(), (long)want.size(), trace.data());
+  if (edges) {   // what the oracle mapped at the edges: [st, en) on rid, with the mate-guided lookup run or not
+    const u32 L = (u32)read_len_base, e = (u32)op.error_threshold, range = (u32)op.max_insert_size;
+    auto tally_edges = [&](u32 rid, u32 st, u32 en, bool looked_up) {
+      const u32 len = (u32)seq[rid].size();
+      if (rid > 0 && st < L + e) ++rs.edge_start;
+      if (en + e + 1 >= len) ++rs.edge_end;
+      if (len < 2 * L) ++rs.short_seq;
+      if (looked_up && rid > 0 && en <= 2 * range) ++rs.lookup_at_start;
+    };
+    if (is_sam) {
+      for (long i = 0; i < n_want_sam; ++i) {
+        const orc_sam_record &w = want_sam[i];
+        tally_edges(w.rid, is_se ? w.pos[0] : std::min(w.pos[0], w.pos[1]), (is_se ? w.end[0] : std::max(w.end[0], w.end[1])) + 1, false);
+      }
+    } else if (mode == MODE_HIC) {
+      for (long i = 0; i < n_want; ++i) {
+        const orc_pairs_record &w = ((const orc_pairs_record *)want.data())[i];
+        tally_edges(w.rid1, w.pos1, w.pos1 + 1, false);
+        tally_edges(w.rid2, w.pos2, w.pos2 + 1, false);
+      }
+    } else {
+      for (long i = 0; i < n_want; ++i) {   // a record for a pair with a mate without candidates of its own: the lookup found it
+        const orc_pair_trace &t = trace[want[i].read_id - first_read_id];
+        const bool looked_up = mode != MODE_SE && (t.supplement_result != 0 || t.n_pos_candidates_gen[0] + t.n_neg_candidates_gen[0] == 0 ||
+                                                   t.n_pos_candidates_gen[1] + t.n_neg_candidates_gen[1] == 0);
+        tally_edges(want[i].rid, want[i].fragment_start, want[i].fragment_start + want[i].fragment_length, looked_up);
+      }
+    }
+  }
   // ---- device objects
   const DevParams P = dev_params(op, K, W);
   const uint32_t *kf; const uint64_t *kk, *kv, *kocc; uint32_t n_occ = 0;
@@ -182,11 +245,12 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   }
   DevIndex ix{};
   ix.slots = slots.data(); ix.n_slots_mask = n_slots_t - 1; ix.shift = 64 - lg; ix.occ = (const u64 *)kocc; ix.n_occ = n_occ; ix.k = K; ix.w = W;
-  std::string refmem(64, '\0');
-  u64 roff[2]; u32 rlen[2];
-  for (int q = 0; q < 2; ++q) { roff[q] = refmem.size(); rlen[q] = (u32)seq[q].size(); refmem += seq[q]; refmem.append(64 + (64 - refmem.size() %% 64) %% 64, '\0'); }
-  refmem.append(128, '\0');
-  DevRef R{(const u8 *)refmem.data(), roff, rlen, 2};
+  // the library's reference layout, in an allocation of exactly its size (AddressSanitizer sees a read past the last padding)
+  std::vector<u64> roff(n_seq);
+  std::vector<u32> rlen(n_seq);
+  std::vector<u8> refmem(ref_layout(n_seq, offs.data(), roff.data()), 0);
+  for (u32 q = 0; q < n_seq; ++q) { rlen[q] = (u32)seq[q].size(); memcpy(refmem.data() + roff[q], seq[q].data(), rlen[q]); }
+  DevRef R{refmem.data(), roff.data(), rlen.data(), n_seq};
   DevBatch B{};
   B.seq1 = (const u8 *)s1.data(); B.off1 = o1.data(); B.seq2 = (const u8 *)s2.data(); B.off2 = o2.data(); B.n_pairs = (u32)n; B.first_read_id = first_read_id;
   std::vector<double> il_(65536); std::vector<int> thr_(96);
@@ -288,15 +352,16 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   return rs;
 }
 
-int main() {
+int main(int argc, char **argv) {
   static_assert(sizeof(OutRecord) == sizeof(orc_pe_record) && sizeof(OutPairs) == sizeof(orc_pe_record), "record layouts");
+  const bool want_edges = argc > 1 && !strcmp(argv[1], "edges");   // the runs at the ends of reference sequences, else all others
   long bad = 0;
   const int mrl = 80;
   const Caps real[3] = {tier_caps(mrl, 0), tier_caps(mrl, 1), tier_caps(mrl, 2)};   // the library's tiers
   const Caps small[3] = {{mrl, 6, 2, 2}, {mrl * 2, 40, 6, 6}, {mrl * 4, 65536, 8192, 8192}};            // most pairs through the CTA kernels, some to the last tier
   const Caps real_long[3] = {tier_caps(150, 0), tier_caps(150, 1), tier_caps(150, 2)};
   const Caps small_long[3] = {{150, 6, 2, 2}, {300, 40, 6, 6}, {600, 65536, 8192, 8192}};
-  struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; Knobs knobs = {}; };
+  struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; Knobs knobs = {}; bool edges = false; };
   const Case cases[] = {
       {"real_tiers", MODE_CHIP, 3, 100, 1, 60, real, mrl},
       {"small_first_tier", MODE_CHIP, 4, 48, 3, 60, small, mrl},
@@ -337,11 +402,25 @@ int main() {
       {"f3_40", MODE_CHIP, 32, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.f0 = 3, .f1 = 40}},
       {"drop20", MODE_CHIP, 33, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.drop_rep = 20}},
       {"min_read_length58", MODE_CHIP, 34, 60, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.min_read_len = 58}},
+      // fragments at the ends of a 50 kbp, a 20 kbp and 45 short sequences (20 bp .. 3 kbp), both strands, every rid
+      {"edges_chip", MODE_CHIP, 40, 400, 1, 60, real, mrl, false, 17, 7, 90, {}, true},
+      {"edges_cta", MODE_CHIP, 41, 160, 2, 60, small, mrl, false, 17, 7, 90, {}, true},
+      {"edges_e1", MODE_CHIP, 42, 160, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.e = 1}, true},
+      {"edges_e15", MODE_CHIP, 43, 320, 1, 60, real, mrl, false, 17, 7, 90, Knobs{.e = 15}, true},
+      {"edges_atac", MODE_ATAC, 44, 160, 1, 60, real, mrl, false, 17, 7, 90, {}, true},
+      {"edges_hic", MODE_HIC, 45, 120, 1, 120, real_long, 150, false, 17, 7, 90, {}, true},
+      {"edges_hic_cta", MODE_HIC, 46, 50, 1, 120, small_long, 150, false, 17, 7, 90, {}, true},
+      {"edges_single_end", MODE_SE, 47, 200, 2, 60, real, mrl, false, 17, 7, 90, {}, true},
+      {"edges_sam", MODE_SAM, 48, 160, 2, 60, real, mrl, false, 17, 7, 90, {}, true},
+      {"edges_sam_single_end", MODE_SAM_SE, 49, 160, 2, 60, real, mrl, false, 17, 7, 90, {}, true},
+      {"edges_f3_40", MODE_CHIP, 50, 300, 2, 60, real, mrl, false, 17, 7, 90, Knobs{.f0 = 3, .f1 = 40}, true},
   };
   const int seed_off = getenv("EMU_SEED_OFFSET") ? atoi(getenv("EMU_SEED_OFFSET")) : 0;   // other inputs of the same kinds (offline fuzzing)
   for (const Case &c : cases) {
-    const RunStats r = run_case(c.mode, c.seed + seed_off, c.n, c.mrl, c.caps, c.max_best, c.len, c.front_only, c.k, c.w, c.fam_copies, c.knobs);
-    printf("%%s: pairs=%%ld records=%%ld tier0=%%ld tier1=%%ld tier2=%%ld bad=%%ld\n", c.name, r.pairs, r.records, r.tier_pairs[0], r.tier_pairs[1], r.tier_pairs[2], r.bad);
+    if (c.edges != want_edges) continue;
+    const RunStats r = run_case(c.mode, c.seed + seed_off, c.n, c.mrl, c.caps, c.max_best, c.len, c.front_only, c.k, c.w, c.fam_copies, c.knobs, c.edges);
+    printf("%%s: pairs=%%ld records=%%ld tier0=%%ld tier1=%%ld tier2=%%ld bad=%%ld edge_start=%%ld edge_end=%%ld short_seq=%%ld lookup_at_start=%%ld\n", c.name, r.pairs, r.records,
+           r.tier_pairs[0], r.tier_pairs[1], r.tier_pairs[2], r.bad, r.edge_start, r.edge_end, r.short_seq, r.lookup_at_start);
     bad += r.bad;
   }
   printf("total_bad=%%ld\n", bad);
@@ -350,7 +429,7 @@ int main() {
 '''
 
 
-def test_device_pipeline_on_emulated_ctas_equals_the_oracle(tmp_path):
+def _run_cases(tmp_path, args=()):
     # CMX_EMU_SANITIZE=address | thread: the same run under AddressSanitizer (out-of-bounds accesses of reads, reference, table,
     # occurrence lists, shared memory) or ThreadSanitizer (the emulation's answer to racecheck: a missing __syncthreads between two
     # phases of a kernel is a data race between the OS threads that play the CUDA threads).  Minutes instead of seconds: on request.
@@ -360,7 +439,7 @@ def test_device_pipeline_on_emulated_ctas_equals_the_oracle(tmp_path):
     if san == "address":
         os.environ["EMU_EXACT_SCRATCH"] = "1"
     env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0", TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0 exitcode=0")
-    out = subprocess.run([str(exe)], capture_output=True, text=True, timeout=7200, env=env)
+    out = subprocess.run([str(exe)] + list(args), capture_output=True, text=True, timeout=7200, env=env)
     assert out.returncode == 0 and "total_bad=0" in out.stdout, out.stdout[-3000:] + out.stderr[-800:]
     if san == "address":
         assert "AddressSanitizer" not in out.stderr, out.stderr[-3000:]
@@ -370,6 +449,11 @@ def test_device_pipeline_on_emulated_ctas_equals_the_oracle(tmp_path):
         reports = out.stderr.split("WARNING: ThreadSanitizer: data race")[1:]
         unexpected = [r for r in reports if not re.search(r"#0 (cluster_kernel|cta_minimizers)\(", r)]
         assert not unexpected, unexpected[0][:3000]
+    return out
+
+
+def test_device_pipeline_on_emulated_ctas_equals_the_oracle(tmp_path):
+    out = _run_cases(tmp_path)
     got = {m.group(1): [int(x) for x in m.groups()[1:]] for m in re.finditer(r"(\w+): pairs=(\d+) records=(\d+) tier0=(\d+) tier1=(\d+) tier2=(\d+)", out.stdout)}
     assert got["real_tiers"][1] > 45 and got["real_tiers"][3] > 5, out.stdout                      # records; pairs that climbed to the second tier
     assert got["small_first_tier"][1] > 30 and got["small_first_tier"][3] > 20 and got["small_first_tier"][4] > 3, out.stdout   # CTA kernels, up to the last tier
@@ -382,3 +466,25 @@ def test_device_pipeline_on_emulated_ctas_equals_the_oracle(tmp_path):
               "f3_40": (30, 4, 0), "drop20": (30, 10, 0), "min_read_length58": (18, 10, 0)}
     for name, (records, tier1, tier2) in floors.items():
         assert got[name][1] > records and got[name][3] >= tier1 and got[name][4] >= tier2, (name, out.stdout)
+
+
+def test_device_pipeline_at_sequence_ends_equals_the_oracle(tmp_path):
+    """Fragments that start or end within 40 bp of a sequence's ends, on every rid of a reference of one 50 kbp, one 20 kbp and
+    45 short sequences (20 bp to 3 kbp, some shorter than k + w - 1, than L + 2e or than a fragment): candidate validity near both
+    ends (valid_cand), the right-end clamp of the verification window, mate-guided lookups whose window begins below a rid's
+    start, negative-strand candidates that wrap below position 0 — every mode, the CTA tiers included.  Each run must map enough at the edges to show it reached them."""
+    out = _run_cases(tmp_path, ["edges"])
+    got = {m.group(1): [int(x) for x in m.groups()[1:]] for m in
+           re.finditer(r"(\w+): pairs=\d+ records=(\d+) tier0=\d+ tier1=(\d+) tier2=(\d+) bad=\d+ edge_start=(\d+) edge_end=(\d+) short_seq=(\d+) lookup_at_start=(\d+)", out.stdout)}
+    # per run, at least: (records, pairs in the second tier, pairs in the last tier, records that start within L + e of a rid > 0's
+    # start, records that end within e + 1 of a sequence's end, records on sequences shorter than 2L, pairs whose mate-guided lookup
+    # window began below a rid > 0's start).  (Single-end, SAM and Hi-C runs have no mate-guided lookup; a Hi-C record holds 5' ends.)
+    floors = {"edges_chip": (130, 90, 0, 30, 3, 3, 4), "edges_cta": (80, 90, 30, 12, 1, 0, 3), "edges_e1": (25, 40, 0, 7, 1, 2, 0),
+              "edges_e15": (90, 70, 0, 9, 1, 0, 3), "edges_atac": (55, 35, 0, 12, 2, 2, 1), "edges_hic": (50, 35, 0, 9, 0, 1, 0),
+              "edges_hic_cta": (15, 30, 8, 6, 0, 5, 0), "edges_single_end": (110, 30, 0, 18, 1, 7, 0), "edges_sam": (70, 30, 0, 12, 2, 1, 0),
+              "edges_sam_single_end": (95, 35, 0, 25, 1, 8, 0), "edges_f3_40": (65, 8, 0, 24, 2, 4, 9)}
+    for name, floor in floors.items():
+        assert all(g >= f for g, f in zip(got[name], floor)), (name, out.stdout)
+    # and over all runs
+    total = [sum(got[name][i] for name in floors) for i in (4, 5, 6)]
+    assert total[0] >= 15 and total[1] >= 35 and total[2] >= 22, (total, out.stdout)

@@ -80,10 +80,19 @@ def revcomp(a):
     return COMP[a[::-1]]
 
 
+def make_short_seqs(rng, n):
+    """n short sequences, as in a scaffold-level assembly: lengths where the mapping rules change for 2x50 and 2x150 reads at
+    -e 8 and 15 (below k + w - 1, around L + 2e, around a fragment), then a spread up to 3 kbp."""
+    lens = [20, 30, 60, 70, 75, 80, 90, 99, 100, 101, 120, 150, 180, 250][:n]
+    lens += [int(x) for x in rng.integers(300, 3001, n - len(lens))]
+    return [ACGT[rng.integers(0, 4, ln)].copy() for ln in lens]
+
+
 def make_reads(rng, seqs, n_pairs, read_len, frag_min=80, frag_max=500, sub_rate=0.01,
                indel_rate=0.001, dup_frac=0.05, short_frac=0.0, n_read_frac=0.002,
-               junk_frac=0.01, chimeric_frac=0.0):
-    """Returns list of (r1, r2) uint8 arrays."""
+               junk_frac=0.01, chimeric_frac=0.0, edge_frac=0.0, edge_rng=None):
+    """Returns list of (r1, r2) uint8 arrays.  A fraction edge_frac of the fragments (drawn from edge_rng) starts within 40 bp of
+    a sequence's start or ends within 40 bp of its end, on any sequence; a fragment longer than its sequence is cut to it."""
     pairs = []
     n_seq = len(seqs)
     lens = np.array([len(s) for s in seqs])
@@ -97,7 +106,16 @@ def make_reads(rng, seqs, n_pairs, read_len, frag_min=80, frag_max=500, sub_rate
                 fl = int(rng.integers(32, 100))
             else:
                 fl = int(rng.integers(frag_min, frag_max + 1))
-            st = int(rng.integers(0, lens[si] - fl))
+            if edge_frac > 0 and edge_rng.random() < edge_frac:
+                si = int(edge_rng.integers(0, n_seq))
+                if fl > lens[si]:
+                    fl = int(edge_rng.integers(min(read_len, lens[si]), lens[si] + 1))
+                d = int(edge_rng.integers(0, min(40, lens[si] - fl) + 1))
+                st = d if edge_rng.random() < 0.5 else int(lens[si]) - fl - d
+            elif lens[si] > fl:
+                st = int(rng.integers(0, lens[si] - fl))
+            else:
+                st, fl = 0, int(lens[si])
             strand = int(rng.integers(0, 2))
             frags.append((si, st, fl, strand))
             if len(frags) > 4096:
@@ -121,6 +139,8 @@ def make_reads(rng, seqs, n_pairs, read_len, frag_min=80, frag_max=500, sub_rate
             # ligation junction: tail of r1 comes from an independent locus
             j = int(rng.integers(30, max(31, read_len - 30)))
             sj = int(rng.integers(0, n_seq))
+            if lens[sj] <= read_len:
+                sj = 0
             pj = int(rng.integers(0, lens[sj] - read_len))
             other = seqs[sj][pj:pj + read_len - j]
             if rng.random() < 0.5:
@@ -181,14 +201,19 @@ def main():
     ap.add_argument("--chimeric-frac", type=float, default=0.0)
     ap.add_argument("--lowercase-frac", type=float, default=0.0)
     ap.add_argument("--barcodes", action="store_true")
+    # edge-heavy inputs (own generator: every other set stays as it was)
+    ap.add_argument("--short-seqs", type=int, default=0, help="short sequences after the --n-seq long ones")
+    ap.add_argument("--edge-frac", type=float, default=0.0, help="fraction of fragments at the ends of sequences")
     a = ap.parse_args()
     os.makedirs(a.out, exist_ok=True)
     rng = np.random.default_rng(a.seed)
     seqs = make_reference(rng, a.n_seq, a.seq_len, a.repeat_len, a.repeat_copies,
                           fam_copies=a.fam_copies, lowercase_frac=a.lowercase_frac)
+    edge_rng = np.random.default_rng([a.seed, 1])
+    seqs += make_short_seqs(edge_rng, a.short_seqs)
     write_fasta(os.path.join(a.out, "ref.fa"), seqs)
     pairs = make_reads(rng, seqs, a.n_pairs, a.read_len, short_frac=a.short_frac,
-                       chimeric_frac=a.chimeric_frac)
+                       chimeric_frac=a.chimeric_frac, edge_frac=a.edge_frac, edge_rng=edge_rng)
     write_fastq(os.path.join(a.out, "read1.fq"), [p[0] for p in pairs], "r", "1")
     write_fastq(os.path.join(a.out, "read2.fq"), [p[1] for p in pairs], "r", "2")
     if a.barcodes:
