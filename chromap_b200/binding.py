@@ -247,6 +247,10 @@ PAIR_TRACE = np.dtype([("n_minimizers", "<i4", 2), ("n_pos_candidates_gen", "<i4
 _lib = None
 
 
+class AllocationStats(C.Structure):  # cmx_allocation_stats
+    _fields_ = [(n, C.c_uint64) for n in ("n_multi", "n_allocated", "n_without_overlap", "n_draws", "n_uni_after", "n_multi_after")]
+
+
 def load_library():
     """Load the CUDA C-ABI library.  Fails loudly when it has not been built — there is no fallback."""
     global _lib
@@ -309,6 +313,8 @@ def load_library():
     L.cmx_upload_barcode_translation.argtypes = [vp, C.POINTER(_Translation)]
     L.cmx_format_bed_bc_tr.restype = i64; L.cmx_format_bed_bc_tr.argtypes = [vp, vp, vp, u64, u32, C.POINTER(_Translation), vp, i64]
     L.cmx_ingest_fastq_range.argtypes = [vp, i32, vp, u64, i32, vp, C.POINTER(ReadRange), C.POINTER(Ingested)]
+    for f in (L.cmx_allocate_multi_mappings_gpu, L.cmx_allocate_multi_mappings):
+        f.argtypes = [vp, vp, vp, u64, C.c_int32, C.c_int32, C.POINTER(u64), C.POINTER(AllocationStats)]
     _lib = L
     return L
 
@@ -590,6 +596,25 @@ class Mapper:
         self._check(self.L.cmx_postprocess_gpu(self.h, recs.ctypes.data, bcs.ctypes.data if bcs is not None else None, len(recs), C.byref(n)),
                     "cmx_postprocess_gpu")
         return recs[:n.value] if bcs is None else (recs[:n.value], bcs[:n.value])
+
+    def _allocate(self, fn, what, recs, bcs, distance, seed):
+        recs = np.ascontiguousarray(recs.copy())
+        if bcs is not None:
+            bcs = np.ascontiguousarray(bcs.copy(), dtype=np.uint64)
+        n = C.c_uint64()
+        st = AllocationStats()
+        self._check(fn(self.h, recs.ctypes.data, bcs.ctypes.data if bcs is not None else None, len(recs), int(distance), int(seed), C.byref(n), C.byref(st)), what)
+        stats = {f: int(getattr(st, f)) for f, _ in AllocationStats._fields_}
+        return recs[:n.value], (bcs[:n.value] if bcs is not None else None), stats
+
+    def allocate_multi_mappings_gpu(self, recs, bcs=None, distance=0, seed=11):
+        """--allocate-multi-mappings on the device: Tn5 / sort / dedup, allocation of the multi-mappings (mapq < 4) to their
+        uni-mapping neighbourhood, sort, MAPQ filter.  Returns (records, barcode keys or None, stats dict)."""
+        return self._allocate(self.L.cmx_allocate_multi_mappings_gpu, "cmx_allocate_multi_mappings_gpu", recs, bcs, distance, seed)
+
+    def allocate_multi_mappings(self, recs, bcs=None, distance=0, seed=11):
+        """Host twin of allocate_multi_mappings_gpu (std::mt19937 + std::discrete_distribution)."""
+        return self._allocate(self.L.cmx_allocate_multi_mappings, "cmx_allocate_multi_mappings", recs, bcs, distance, seed)
 
     def postprocess_pairs(self, recs):
         recs = np.ascontiguousarray(recs.copy())

@@ -11,6 +11,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <memory>
+#include <random>
 #include <string>
 #include <thread>
 #include <tuple>
@@ -18,6 +19,7 @@
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <thrust/iterator/counting_iterator.h>
 
 #include "../../include/chromap_b200.h"
 #include "cuda_owners.cuh"
@@ -27,6 +29,7 @@
 #include "cta_pair_candidates.cuh"
 #include "cta_verify_pairing.cuh"
 #include "postprocess.cuh"
+#include "allocate.cuh"
 #include "exchange.cuh"
 #include "sam_kernels.cuh"
 #include "ingest.cuh"
@@ -1260,11 +1263,17 @@ static inline void tn5_se(cmx_pe_record &r) {  // single-end, bed_mapping.h:97-1
   if (r.direction == 1) r.fragment_start += 4; else r.fragment_length -= 5;
 }
 
+// cmx_postprocess / cmx_postprocess_bc under given parameters (the allocation runs them twice with others than the context's)
+static void postprocess_host(const cmx_params &p, cmx_pe_record *recs, uint64_t n, uint64_t *n_out);
+static void postprocess_bc_host(const cmx_params &p, cmx_pe_record *recs, uint64_t *bcs, uint64_t n, uint64_t *n_out);
 int cmx_postprocess(cmx_ctx *ctx, cmx_pe_record *recs, uint64_t n, uint64_t *n_out) {
   if (!ctx || (!recs && n) || !n_out) return CMX_ERR_INVALID;
-  const cmx_params &p = ctx->params;
+  postprocess_host(ctx->params, recs, n, n_out);
+  return CMX_OK;
+}
+static void postprocess_host(const cmx_params &p, cmx_pe_record *recs, uint64_t n, uint64_t *n_out) {
   *n_out = 0;
-  if (n == 0) return CMX_OK;
+  if (n == 0) return;
   auto less = [](const cmx_pe_record &a, const cmx_pe_record &b) { return rec_key(a) < rec_key(b); };
   const bool se = p.single_end != 0;  // single-end duplicates: same start on the same sequence (bed_mapping.h:89-92)
   auto same = [se](const cmx_pe_record &a, const cmx_pe_record &b) {
@@ -1289,7 +1298,7 @@ int cmx_postprocess(cmx_ctx *ctx, cmx_pe_record *recs, uint64_t n, uint64_t *n_o
       i = j;
     }
     *n_out = o;
-    return CMX_OK;
+    return;
   }
   if (p.tn5_shift) for (uint64_t i = 0; i < n; ++i) tn5(recs[i]);  // chromap.h:1322-1355
   std::sort(recs, recs + n, less);
@@ -1307,7 +1316,6 @@ int cmx_postprocess(cmx_ctx *ctx, cmx_pe_record *recs, uint64_t n, uint64_t *n_o
   }
   for (uint64_t i = 0; i < n; ++i) if (recs[i].mapq >= p.mapq_threshold) recs[o++] = recs[i];
   *n_out = o;
-  return CMX_OK;
 }
 
 int cmx_postprocess_pairs(cmx_ctx *ctx, cmx_pairs_record *recs, uint64_t n, uint64_t *n_out) {
@@ -1356,9 +1364,12 @@ int64_t cmx_format_pairs(const char *const *names, const uint32_t *lengths, uint
 
 int cmx_postprocess_bc(cmx_ctx *ctx, cmx_pe_record *recs, uint64_t *bcs, uint64_t n, uint64_t *n_out) {
   if (!ctx || (n && (!recs || !bcs)) || !n_out) return CMX_ERR_INVALID;
-  const cmx_params &p = ctx->params;
+  postprocess_bc_host(ctx->params, recs, bcs, n, n_out);
+  return CMX_OK;
+}
+static void postprocess_bc_host(const cmx_params &p, cmx_pe_record *recs, uint64_t *bcs, uint64_t n, uint64_t *n_out) {
   *n_out = 0;
-  if (n == 0) return CMX_OK;
+  if (n == 0) return;
   std::vector<cmx_pe_record> rr(recs, recs + n);
   std::vector<uint64_t> bb(bcs, bcs + n);
   if (!p.low_memory_mode && p.tn5_shift) for (auto &r : rr) { if (p.single_end) tn5_se(r); else tn5(r); }
@@ -1392,7 +1403,6 @@ int cmx_postprocess_bc(cmx_ctx *ctx, cmx_pe_record *recs, uint64_t *bcs, uint64_
     i = j;
   }
   *n_out = o;
-  return CMX_OK;
 }
 
 int64_t cmx_format_bed_bc(const char *const *names, const cmx_pe_record *recs, const uint64_t *bcs, uint64_t n, uint32_t bc_len, char *buf, int64_t cap) {
@@ -1496,6 +1506,208 @@ int cmx_postprocess_gpu(cmx_ctx *ctx, void *records, uint64_t *barcode_keys, uin
   if (bc && nsel) CU(cudaMemcpyAsync(barcode_keys, d_bcb, nsel * 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   *n_out = nsel;
+  return CMX_OK;
+}
+
+// ---- --allocate-multi-mappings (allocate.cuh) ------------------------------------------------------------------------------
+// The checks both entries make before touching the records
+static int allocation_refusal(cmx_ctx *ctx, const char *who, const cmx_pe_record *records, uint64_t n, int32_t distance, uint64_t *n_out) {
+  if (!ctx || (!records && n) || !n_out) return CMX_ERR_INVALID;
+  const cmx_params &p = ctx->params;
+  if (p.low_memory_mode) return fail(ctx, CMX_ERR_INVALID, "%s: a low-memory context never allocates multi-mappings (the reference skips the step there)", who);
+  if (p.output_format == 4 || p.output_format == 5)
+    return fail(ctx, CMX_ERR_INVALID, "%s: multi-mapping allocation covers BED / TagAlign records, not SAM or pairs", who);
+  if (distance < 0) return fail(ctx, CMX_ERR_INVALID, "%s: distance %d < 0 (the reference's uint32 cast would turn it into a wrap-around)", who, distance);
+  if (n > 0x7FFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "%s: more than 2^31-1 records in one call", who);
+  return CMX_OK;
+}
+static const char *NO_MULTI = "%s: no multi-mapping (mapq < 4) among the records; the reference aborts here (mapping_processor.h:375)";
+
+int cmx_allocate_multi_mappings(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_keys, uint64_t n, int32_t distance, int32_t seed,
+                                uint64_t *n_out, cmx_allocation_stats *stats) {
+  const char *who = "cmx_allocate_multi_mappings";
+  const int rc = allocation_refusal(ctx, who, records, n, distance, n_out);
+  if (rc) return rc;
+  const cmx_params &p = ctx->params;
+  const bool bc = barcode_keys != nullptr;
+  std::vector<cmx_pe_record> rr(records, records + n);
+  std::vector<uint64_t> bb(bc ? barcode_keys : nullptr, bc ? barcode_keys + n : nullptr);
+  cmx_params p1 = p;  // Tn5, sort, dedup; the MAPQ filter comes after the allocation
+  p1.mapq_threshold = 0;
+  uint64_t n1 = 0;
+  if (bc) postprocess_bc_host(p1, rr.data(), bb.data(), n, &n1); else postprocess_host(p1, rr.data(), n, &n1);
+  // uni records per sequence: starts (sorted: the records are) and ends in that order, ends sorted
+  std::vector<uint8_t> keep(n1, 0);
+  std::vector<uint64_t> us, ue_s;
+  std::vector<uint32_t> multi;
+  for (uint64_t i = 0; i < n1; ++i) {
+    const uint64_t rid = (uint64_t)rr[i].rid << 32;
+    if (rr[i].mapq < 4) { multi.push_back((uint32_t)i); continue; }
+    keep[i] = 1;
+    us.push_back(rid | rr[i].fragment_start);
+    ue_s.push_back(rid | (uint32_t)(rr[i].fragment_start + rr[i].fragment_length));
+  }
+  if (multi.empty()) return fail(ctx, CMX_ERR_INVALID, NO_MULTI, who);
+  std::vector<uint64_t> ue = ue_s;
+  std::sort(ue.begin(), ue.end());
+  std::stable_sort(multi.begin(), multi.end(), [&](uint32_t a, uint32_t b) { return rr[a].read_id < rr[b].read_id; });
+  auto weight = [&](const cmx_pe_record &r) -> uint32_t {  // mapping_processor.h:255-317
+    const uint64_t rid = (uint64_t)r.rid << 32;
+    const uint32_t d = (uint32_t)distance, start = r.fragment_start, end = start + r.fragment_length;
+    const uint32_t qs = start > d ? start - d : 0u, qe = end + d;
+    const uint64_t lo = std::lower_bound(us.begin(), us.end(), rid) - us.begin(), a = std::lower_bound(us.begin(), us.end(), rid | qe) - us.begin();
+    if (qe > qs)
+      return (uint32_t)((a - lo) - (uint64_t)(std::lower_bound(ue.begin(), ue.end(), rid | (qs + 1u)) - std::lower_bound(ue.begin(), ue.end(), rid)));
+    uint32_t c = 0;  // end + d wrapped: only uni records starting within AL_MAX_LEN of qs can end past it
+    const uint64_t i0 = std::max<uint64_t>(lo, std::lower_bound(us.begin(), us.end(), rid | (qs > AL_MAX_LEN ? qs - AL_MAX_LEN : 0u)) - us.begin());
+    for (uint64_t i = i0; i < a; ++i) c += (uint32_t)ue_s[i] > qs;
+    return c;
+  };
+  std::mt19937 generator(seed);
+  cmx_allocation_stats st{};
+  st.n_multi = multi.size();
+  std::vector<uint32_t> weights;
+  for (size_t s = 0; s < multi.size();) {  // one read: candidates multi[s, e)
+    size_t e = s;
+    uint32_t sum = 0;
+    weights.clear();
+    for (; e < multi.size() && rr[multi[e]].read_id == rr[multi[s]].read_id; ++e) { weights.push_back(weight(rr[multi[e]])); sum += weights.back(); }
+    if (sum == 0) ++st.n_without_overlap;
+    else {
+      std::discrete_distribution<uint32_t> distribution(weights.begin(), weights.end());
+      keep[multi[s + distribution(generator)]] = 1;
+      ++st.n_allocated;
+      st.n_draws += weights.size() >= 2;
+    }
+    s = e;
+  }
+  uint64_t n2 = 0;
+  for (uint64_t i = 0; i < n1; ++i)
+    if (keep[i]) { rr[n2] = rr[i]; if (bc) bb[n2] = bb[i]; ++n2; }
+  for (uint64_t i = 0; i < n2; ++i) { if (rr[i].is_unique == 1) ++st.n_uni_after; else ++st.n_multi_after; }
+  cmx_params p2 = p;  // sort again, MAPQ filter
+  p2.remove_pcr_duplicates = 0; p2.tn5_shift = 0;
+  uint64_t n3 = 0;
+  if (bc) postprocess_bc_host(p2, rr.data(), bb.data(), n2, &n3); else postprocess_host(p2, rr.data(), n2, &n3);
+  std::copy(rr.begin(), rr.begin() + n3, records);
+  if (bc) std::copy(bb.begin(), bb.begin() + n3, barcode_keys);
+  *n_out = n3;
+  if (stats) *stats = st;
+  return CMX_OK;
+}
+
+int cmx_allocate_multi_mappings_gpu(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_keys, uint64_t n, int32_t distance, int32_t seed,
+                                    uint64_t *n_out, cmx_allocation_stats *stats) {
+  const char *who = "cmx_allocate_multi_mappings_gpu";
+  const int rc0 = allocation_refusal(ctx, who, records, n, distance, n_out);
+  if (rc0) return rc0;
+  if (n == 0) return fail(ctx, CMX_ERR_INVALID, NO_MULTI, who);
+  CU(cudaSetDevice(ctx->device));
+  const cmx_params &p = ctx->params;
+  const bool bc = barcode_keys != nullptr;
+  PpParams P;
+  P.kind = bc ? PP_BED_BC : (p.single_end ? PP_BED_SE : PP_BED);
+  P.low_mem = 0; P.dedup = p.remove_pcr_duplicates; P.tn5 = p.tn5_shift; P.mapq_threshold = 0; P.se = p.single_end;
+  cudaStream_t st = ctx->stream;
+  DevMem<PpRecord> d_a, d_b;
+  DevMem<u64> d_bca, d_bcb;
+  CU(d_a.alloc(n * sizeof(PpRecord))); CU(d_b.alloc(n * sizeof(PpRecord)));
+  if (bc) { CU(d_bca.alloc(n * 8)); CU(d_bcb.alloc(n * 8)); }
+  CU(cudaMemcpyAsync(d_a, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
+  if (bc) CU(cudaMemcpyAsync(d_bca, barcode_keys, n * 8, cudaMemcpyHostToDevice, st));
+  u64 n1 = 0;
+  int rc = pp_device(ctx, P, d_a, d_bca, n, d_b, d_bcb, &n1);  // sorted, deduplicated: d_b[0, n1)
+  if (rc != CMX_OK) return rc;
+  // 1. split
+  DevMem<u8> d_uni, d_multi;
+  DevMem<u64> d_ks, d_ke, d_us, d_ue_s, d_ue, d_cnt;
+  DevMem<u32> d_midx;
+  DevMem<> d_tmp;
+  CU(d_uni.alloc(n1 + 1)); CU(d_multi.alloc(n1 + 1)); CU(d_ks.alloc(n1 * 8)); CU(d_ke.alloc(n1 * 8));
+  CU(d_us.alloc(n1 * 8)); CU(d_ue_s.alloc(n1 * 8)); CU(d_ue.alloc(n1 * 8)); CU(d_midx.alloc(n1 * 4)); CU(d_cnt.alloc(32));
+  const unsigned nb1 = (unsigned)((n1 + 255) / 256);
+  al_split_kernel<<<nb1, 256, 0, st>>>(d_b, n1, d_uni, d_multi, d_ks, d_ke);
+  thrust::counting_iterator<u32> iota(0u);
+  size_t tmp_bytes = 0, need = 0;
+  CU(cub::DeviceSelect::Flagged(nullptr, need, d_ks.p, d_uni.p, d_us.p, d_cnt.p, (int)n1, st)); tmp_bytes = std::max(tmp_bytes, need);
+  CU(cub::DeviceSelect::Flagged(nullptr, need, iota, d_multi.p, d_midx.p, d_cnt.p, (int)n1, st)); tmp_bytes = std::max(tmp_bytes, need);
+  CU(cub::DeviceRadixSort::SortKeys(nullptr, need, d_ue_s.p, d_ue.p, (int)n1, 0, 64, st)); tmp_bytes = std::max(tmp_bytes, need);
+  CU(cub::DeviceRadixSort::SortPairs(nullptr, need, (u32 *)nullptr, (u32 *)nullptr, (u32 *)nullptr, (u32 *)nullptr, (int)n1, 0, 32, st)); tmp_bytes = std::max(tmp_bytes, need);
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, need, (u32 *)nullptr, (u32 *)nullptr, (int)n1, st)); tmp_bytes = std::max(tmp_bytes, need);
+  CU(cub::DeviceSelect::Flagged(nullptr, need, d_b.p, d_uni.p, d_a.p, d_cnt.p, (int)n1, st)); tmp_bytes = std::max(tmp_bytes, need);
+  CU(cub::DeviceSelect::Flagged(nullptr, need, d_bcb.p, d_uni.p, d_bca.p, d_cnt.p, (int)n1, st)); tmp_bytes = std::max(tmp_bytes, need);
+  CU(d_tmp.alloc(tmp_bytes));
+  CU(cudaMemsetAsync(d_cnt, 0, 32, st));
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_ks.p, d_uni.p, d_us.p, d_cnt.p, (int)n1, st));
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_ke.p, d_uni.p, d_ue_s.p, d_cnt.p, (int)n1, st));
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, iota, d_multi.p, d_midx.p, d_cnt + 1, (int)n1, st));
+  u64 cnt[2] = {0, 0};
+  CU(cudaMemcpyAsync(cnt, d_cnt, 16, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const u32 n_uni = (u32)cnt[0], m = (u32)cnt[1];
+  if (m == 0) return fail(ctx, CMX_ERR_INVALID, NO_MULTI, who);
+  // 2. weights
+  if (n_uni) CU(cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, d_ue_s.p, d_ue.p, (int)n_uni, 0, 64, st));
+  DevMem<u32> d_w, d_rk, d_rk2, d_j, d_perm, d_ws, d_rs, d_draws, d_didx, d_stream;
+  DevMem<u8> d_head, d_kept;
+  CU(d_w.alloc(m * 4ull)); CU(d_rk.alloc(m * 4ull)); CU(d_rk2.alloc(m * 4ull)); CU(d_j.alloc(m * 4ull)); CU(d_perm.alloc(m * 4ull));
+  CU(d_ws.alloc(m * 4ull)); CU(d_rs.alloc(m * 4ull)); CU(d_draws.alloc(m * 4ull)); CU(d_didx.alloc(m * 4ull)); CU(d_head.alloc(m)); CU(d_kept.alloc(m));
+  const unsigned nbm = (m + 255) / 256;
+  al_count_kernel<<<nbm, 256, 0, st>>>(d_b, d_midx, m, d_us, d_ue_s, d_ue, n_uni, (u32)distance, d_w, d_rk);
+  CU(cudaGetLastError());
+  // 3. group by read (stable), heads, per read counts, draw indices
+  pp_iota_kernel<<<nbm, 256, 0, st>>>(d_j, m);
+  CU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_rk.p, d_rk2.p, d_j.p, d_perm.p, (int)m, 0, 32, st));
+  al_head_kernel<<<nbm, 256, 0, st>>>(d_rk2, d_perm, d_w, m, d_head, d_ws);
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, iota, d_head.p, d_rs.p, d_cnt + 2, (int)m, st));
+  CU(cudaMemcpyAsync(cnt, d_cnt + 2, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const u32 n_reads = (u32)cnt[0];
+  const unsigned nbr = (n_reads + 255) / 256;
+  al_read_kernel<<<nbr, 256, 0, st>>>(d_rs, n_reads, m, d_ws, d_draws, d_kept);
+  CU(cudaGetLastError());
+  CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_draws.p, d_didx.p, (int)n_reads, st));
+  u32 last[2] = {0, 0};
+  CU(cudaMemcpyAsync(&last[0], d_didx + (n_reads - 1), 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(&last[1], d_draws + (n_reads - 1), 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const u64 n_draws = (u64)last[0] + last[1];
+  // 4. the generator stream
+  if (n_draws) {
+    std::vector<u32> mt(624);
+    mt_seed_fill(mt.data(), (u32)seed);
+    DevMem<u32> d_mt;
+    CU(d_mt.alloc(624 * 4)); CU(d_stream.alloc(2 * n_draws * 4));
+    CU(cudaMemcpyAsync(d_mt, mt.data(), 624 * 4, cudaMemcpyHostToDevice, st));
+    al_mt_kernel<<<1, 256, 0, st>>>(d_mt, 2 * n_draws, d_stream);
+    CU(cudaStreamSynchronize(st));  // d_mt's host copy lives in this block
+  }
+  // 5. the draws: keep = uni flags + picked candidates
+  al_draw_kernel<<<nbr, 256, 0, st>>>(d_rs, n_reads, m, d_ws, d_perm, d_midx, d_draws, d_didx, d_kept, d_stream, d_uni);
+  CU(cudaGetLastError());
+  // 6. compact into d_a, count is_unique, sort again and filter
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_b.p, d_uni.p, d_a.p, d_cnt + 3, (int)n1, st));
+  if (bc) CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_bcb.p, d_uni.p, d_bca.p, d_cnt + 3, (int)n1, st));
+  CU(cudaMemcpyAsync(cnt, d_cnt + 3, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const u64 n2 = cnt[0];
+  CU(cudaMemsetAsync(d_cnt + 3, 0, 8, st));
+  if (n2) al_unique_count_kernel<<<(unsigned)((n2 + 255) / 256), 256, 0, st>>>(d_a, n2, (unsigned long long *)(d_cnt.p + 3));  // n2 == 0: no uni record, no read kept
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(cnt + 1, d_cnt + 3, 8, cudaMemcpyDeviceToHost, st));
+  P.dedup = 0; P.tn5 = 0; P.mapq_threshold = p.mapq_threshold;
+  u64 n3 = 0;
+  rc = pp_device(ctx, P, d_a, d_bca, n2, d_b, d_bcb, &n3);  // waits for the stream
+  if (rc != CMX_OK) return rc;
+  if (n3) CU(cudaMemcpyAsync(records, d_b, n3 * sizeof(PpRecord), cudaMemcpyDeviceToHost, st));
+  if (bc && n3) CU(cudaMemcpyAsync(barcode_keys, d_bcb, n3 * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  *n_out = n3;
+  if (stats) {
+    stats->n_multi = m; stats->n_allocated = n2 - n_uni; stats->n_without_overlap = n_reads - (n2 - n_uni); stats->n_draws = n_draws;
+    stats->n_uni_after = cnt[1]; stats->n_multi_after = n2 - cnt[1];
+  }
   return CMX_OK;
 }
 

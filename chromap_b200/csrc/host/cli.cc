@@ -367,6 +367,8 @@ struct Options {
   cmx_params p;
   std::string ref_path, index_path, r1_path, r2_path, out_path, bc_path, wl_path, tr_path;
   int k = 17, w = 7, bc_err = 1, out_nw = 0;
+  bool allocate = false;                    // --allocate-multi-mappings (in-memory runs only, as the reference)
+  int alloc_distance = 0, alloc_seed = 11;  // --multi-mapping-allocation-distance / -seed (mapping_parameters.h)
   double bc_prob = 0.9;
   bool build_index = false, skip_bc_check = false, host_reader = false, paf = false;
   bool cell_level_dedup = false;  // remove_pcr_duplicates_at_bulk_level == false (mapping_parameters.h:49; --preset atac clears it)
@@ -397,7 +399,13 @@ static Options ParseOptions(int argc, char **argv) {
              "  --barcode-translate FILE  write barcoded BED fields through a TO,FROM (or TO<tab>FROM) table, plain or gzipped, as chromap\n"
              "                      (e.g. ATAC to gene-expression barcodes of 10x Multiome); bulk runs ignore it\n"
              "  --bc-error-threshold INT  max Hamming distance allowed to correct a barcode against the whitelist: 0, 1 or 2 [1]\n"
-             "  --bc-probability-threshold FLT  min probability of the best correction among the candidates [0.9]\n");
+             "  --bc-probability-threshold FLT  min probability of the best correction among the candidates [0.9]\n"
+             "  --allocate-multi-mappings  give each multi-mapped read (MAPQ < 4) one of its mappings, drawn with weights = the\n"
+             "                      uni-mappings near it; reads with none nearby are dropped (in-memory BED / TagAlign runs; --low-mem\n"
+             "                      and the presets ignore it)\n"
+             "  --multi-mapping-allocation-distance INT  uni-mappings within this distance from any end of multi-mappings are used\n"
+             "                      for allocation [0]\n"
+             "  --multi-mapping-allocation-seed INT  seed for random number generator in multi-mapping allocation [11]\n");
       exit(0);
     }
     else if (a == "-v" || a == "--version") { fprintf(stderr, "chromap-b200 0.1 (parity target: chromap 0.3.3-r521)\n"); exit(0); }
@@ -439,7 +447,10 @@ static Options ParseOptions(int argc, char **argv) {
     else if (a == "-t" || a == "--num-threads" || a == "--cache-size" || a == "--cache-update-param" || a == "--frip-est-params" || a == "--k-for-minhash" || a == "-A" || a == "--match-score" ||
              a == "-B" || a == "--mismatch-penalty" || a == "-O" || a == "--gap-open-penalties" || a == "-E" || a == "--gap-extension-penalties") val();
     else if (a == "--BED" || a == "--debug-cache" || a == "--turn-off-num-uniq-cache-slots") {}
-    else if (a == "--chr-order" || a == "--pairs-natural-chr-order" || a == "--allocate-multi-mappings" ||
+    else if (a == "--allocate-multi-mappings") o.allocate = true;
+    else if (a == "--multi-mapping-allocation-distance") o.alloc_distance = atoi(val().c_str());
+    else if (a == "--multi-mapping-allocation-seed") o.alloc_seed = atoi(val().c_str());
+    else if (a == "--chr-order" || a == "--pairs-natural-chr-order" ||
              a == "-p" || a == "--matrix-output-prefix")
       Die("chromap-b200: option " + a + " changes the output in ways that are not on the GPU path; use the reference chromap for it");
     else if (a == "--TagAlign") p.output_format = 2;  // same records as BED, TagAlign / PairedTagAlign text (chromap_driver.cc:417-418)
@@ -499,6 +510,14 @@ static void CheckMappingOptions(const Options &o) {
   if (o.sc && o.p.remove_pcr_duplicates && o.p.low_memory_mode && !o.cell_level_dedup)  // mapping_writer.h:254-262: only the low-memory merge has the bulk-level variant
     Die("chromap-b200: bulk-level duplicate removal of barcoded data is not on the GPU path (use --preset atac or --remove-pcr-duplicates-at-cell-level)");
   if (o.out_path.empty()) Die("No output file specified!");
+  if (o.allocate && !o.p.low_memory_mode) {  // low-memory runs accept the option and never allocate (chromap.h:605-613)
+    if (o.alloc_distance < 0)
+      Die("chromap-b200: --multi-mapping-allocation-distance " + std::to_string(o.alloc_distance) + ": use 0 or more; the reference casts a negative distance " +
+          "to uint32, so its result is an accident of wrap-around, and the GPU path refuses it");
+    if (o.sam || o.paf || o.pairs)
+      Die("chromap-b200: --allocate-multi-mappings goes with BED / TagAlign output on the GPU path, not with --SAM, --PAF or --pairs");
+  }
+  if (o.allocate) fprintf(stderr, "Will allocate multi-mappings after mapping.\n");  // chromap_driver.cc:610-611
 }
 // What a mapping run holds from start-up to exit: device context, reference, translation table, raw read files, record buffer
 struct Session {
@@ -720,6 +739,20 @@ template <class D, class H> static int64_t FormatOnDeviceElseHost(cmx_ctx *ctx, 
   if (bytes == CMX_ERR_BARCODE_TRANSLATE) DieBarcodeNotTranslated("a barcode segment has no entry in the translation table");
   return bytes;
 }
+// --allocate-multi-mappings in an in-memory run: post-processing with the allocation on the device, its host twin if the device
+// call fails for memory; the reference's log lines (mapping_processor.h:363,431-435, chromap.h:1348-1350).  A run without any
+// multi-mapping ends here, before the output file is created (the reference aborts on an assertion).
+static void Allocate(const Options &o, cmx_ctx *ctx, std::vector<cmx_pe_record> &all, uint64_t *bc, uint64_t *keep) {
+  const double t0 = Now();
+  cmx_allocation_stats st{};
+  int rc = cmx_allocate_multi_mappings_gpu(ctx, all.data(), bc, all.size(), o.alloc_distance, o.alloc_seed, keep, &st);
+  if (rc == CMX_ERR_CUDA) rc = cmx_allocate_multi_mappings(ctx, all.data(), bc, all.size(), o.alloc_distance, o.alloc_seed, keep, &st);
+  if (rc) Die(std::string("chromap-b200: ") + cmx_last_error(ctx) + "; no output file is written");
+  fprintf(stderr, "Got all %llu multi-mappings!\nAllocated %llu multi-mappings in %.2fs.\n# multi-mappings that have no uni-mapping overlaps: %llu.\n",
+          (unsigned long long)st.n_multi, (unsigned long long)st.n_allocated, Now() - t0, (unsigned long long)st.n_without_overlap);
+  fprintf(stderr, "After allocating multi-mappings, # uni-mappings: %llu, # multi-mappings: %llu, total: %llu.\n", (unsigned long long)st.n_uni_after,
+          (unsigned long long)st.n_multi_after, (unsigned long long)(st.n_uni_after + st.n_multi_after));
+}
 // Post-processing (sort / dedup / filter on the device; the host routine if the records do not fit beside the index), text, file
 static void WriteOutput(const Options &o, uint32_t bc_len, Session *s, Mapped *m, double t_start) {
   cmx_ctx *ctx = s->ctx;
@@ -731,6 +764,7 @@ static void WriteOutput(const Options &o, uint32_t bc_len, Session *s, Mapped *m
   for (const auto &x : m->names1) n1.push_back(x.c_str());
   for (const auto &x : m->names2) n2.push_back(x.c_str());
   std::vector<cmx_pe_record> &all = m->all;
+  const bool allocate = o.allocate && !o.p.low_memory_mode;
   uint64_t keep = 0;
   std::vector<char> text;
   int64_t bytes = 0;
@@ -753,13 +787,15 @@ static void WriteOutput(const Options &o, uint32_t bc_len, Session *s, Mapped *m
         ctx, &text, [&](char *buf, int64_t cap) { return cmx_format_pairs_gpu(ctx, names.data(), lens.data(), (uint32_t)names.size(), pr, keep, n1.data(), n1.size(), 0, buf, cap); },
         [&](char *buf, int64_t cap) { return cmx_format_pairs(names.data(), lens.data(), (uint32_t)names.size(), pr, keep, n1.data(), 0, buf, cap); });
   } else if (o.sc) {
-    if (cmx_postprocess_gpu(ctx, all.data(), m->bc.data(), all.size(), &keep) && cmx_postprocess_bc(ctx, all.data(), m->bc.data(), all.size(), &keep)) Die(cmx_last_error(ctx));
+    if (allocate) Allocate(o, ctx, all, m->bc.data(), &keep);
+    else if (cmx_postprocess_gpu(ctx, all.data(), m->bc.data(), all.size(), &keep) && cmx_postprocess_bc(ctx, all.data(), m->bc.data(), all.size(), &keep)) Die(cmx_last_error(ctx));
     bytes = FormatOnDeviceElseHost(  // the host twin without a table is exactly cmx_format_bed_bc
         ctx, &text, [&](char *buf, int64_t cap) { return cmx_format_bed_gpu(ctx, names.data(), all.data(), m->bc.data(), keep, bc_len, buf, cap); },
         [&](char *buf, int64_t cap) { return cmx_format_bed_bc_tr(names.data(), all.data(), m->bc.data(), keep, bc_len, o.tr_path.empty() ? nullptr : &s->tr, buf, cap); });
     fprintf(stderr, "Number of barcodes in whitelist: %llu.\nNumber of corrected barcodes: %llu.\n", (unsigned long long)m->n_bc_in, (unsigned long long)m->n_bc_cor);
   } else {
-    if (cmx_postprocess_gpu(ctx, all.data(), nullptr, all.size(), &keep) && cmx_postprocess(ctx, all.data(), all.size(), &keep)) Die(cmx_last_error(ctx));
+    if (allocate) Allocate(o, ctx, all, nullptr, &keep);
+    else if (cmx_postprocess_gpu(ctx, all.data(), nullptr, all.size(), &keep) && cmx_postprocess(ctx, all.data(), all.size(), &keep)) Die(cmx_last_error(ctx));
     if (o.tagalign && !o.se)  // PairedTagAlign: two lines per pair (host formatter); single-end TagAlign is the BED text
       bytes = Format(&text, [&](char *buf, int64_t cap) { return cmx_format_tagalign(names.data(), all.data(), keep, buf, cap); });
     else

@@ -23,11 +23,13 @@ inline void mapq_tables_fill(double *inv_log, int *pen_thr) {
     pen_thr[v] = (int)lo;
   }
 }
-// select_kernel's mt_init: the 624-word state of std::mt19937(11) right after seeding.
-inline void mt_init_fill(u32 *mt) {
-  mt[0] = 11u;
+// The 624-word state of std::mt19937(seed) right after seeding (an int seed is reduced mod 2^32, random.tcc seed()).
+inline void mt_seed_fill(u32 *mt, u32 seed) {
+  mt[0] = seed;
   for (int i = 1; i < 624; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (u32)i;
 }
+// select_kernel's mt_init: std::mt19937(11).
+inline void mt_init_fill(u32 *mt) { mt_seed_fill(mt, 11u); }
 
 struct Counters {  // device-side statistics (atomics)
   u64 n_minimizers, n_probe_steps, n_found, n_occ_reads, n_verified, n_candidates, n_mapped, n_unique, n_overflow;

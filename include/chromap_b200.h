@@ -194,6 +194,27 @@ int cmx_postprocess_bc(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_k
  * is NULL for bulk data.  Replaces the sort / merge of mapping_processor.h:100-202 and mapping_writer.h:166-376 the
  * same way; results are identical to the host routines.  n < 2^31 per call. */
 int cmx_postprocess_gpu(cmx_ctx *ctx, void *records, uint64_t *barcode_keys, uint64_t n, uint64_t *n_out);
+
+/* --allocate-multi-mappings: counts of one call (the reference's log lines, mapping_processor.h:363,431-435,502-504). */
+typedef struct {
+  uint64_t n_multi;            /* multi-mappings (mapq < 4) after duplicate removal: "Got all X multi-mappings!" */
+  uint64_t n_allocated;        /* reads given one of their candidates */
+  uint64_t n_without_overlap;  /* reads whose weight sum is 0 (dropped) */
+  uint64_t n_draws;            /* reads that consumed two generator outputs (>= 2 candidates, non-zero sum) */
+  uint64_t n_uni_after, n_multi_after;  /* is_unique split of the allocated set, before the MAPQ filter */
+} cmx_allocation_stats;
+/* In-memory post-processing with multi-mapping allocation (chromap.h:1322-1355 with allocate_multi_mappings): Tn5 shift, sort,
+ * duplicate removal (keeping the last of a run), AllocateMultiMappings (mapping_processor.h:319-440: each read with mapq < 4
+ * keeps one candidate drawn with weights = the uni-mappings within `distance` of it, from one std::mt19937(seed); reads
+ * without any such uni-mapping are dropped), sort, MAPQ filter.  Bulk or barcoded (barcode_keys != NULL), paired-end or
+ * single-end records, in place on host buffers like cmx_postprocess_gpu; *n_out = the records left.  CMX_ERR_INVALID, with
+ * the reason in cmx_last_error() and the records untouched, for a low-memory context (the reference never allocates there),
+ * a pairs or SAM context, distance < 0, n >= 2^31, or a record set without any multi-mapping (the reference aborts). */
+int cmx_allocate_multi_mappings_gpu(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_keys, uint64_t n,
+                                    int32_t distance, int32_t seed, uint64_t *n_out, cmx_allocation_stats *stats);
+/* Host twin (std::mt19937 + std::discrete_distribution): the same results, refusals and counts. */
+int cmx_allocate_multi_mappings(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_keys, uint64_t n,
+                                int32_t distance, int32_t seed, uint64_t *n_out, cmx_allocation_stats *stats);
 int64_t cmx_format_bed_bc(const char *const *names, const cmx_pe_record *records, const uint64_t *barcode_keys, uint64_t n, uint32_t bc_len,
                           char *buf, int64_t cap);
 /* BED text (mapping_writer.cc:75-83); names = n_seq C strings.  Returns bytes (or needed size if buf NULL). */
