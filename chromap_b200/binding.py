@@ -32,8 +32,32 @@ class ReadSet(C.Structure):
     _fields_ = [("names", C.c_void_p), ("seq", C.c_void_p), ("off", C.c_void_p), ("qual", C.c_void_p)]
 
 
+def _sam_read_set(r, keep):
+    """cmx_read_set of (names, seqs, quals) lists of bytes (quals may be None); keep holds the buffers alive."""
+    if r is None:
+        return None
+    nm, sq, ql = r
+    arr = (C.c_char_p * len(nm))(*nm)
+    seq = np.frombuffer(b"".join(sq), dtype=np.uint8)
+    off = np.zeros(len(sq) + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([len(x) for x in sq])
+    qual = np.frombuffer(b"".join(ql), dtype=np.uint8) if ql is not None else None
+    keep.extend([arr, seq, off, qual])
+    return ReadSet(C.cast(arr, C.c_void_p), seq.ctypes.data, off.ctypes.data, qual.ctypes.data if qual is not None else None)
+
+
 def format_sam(params, ref_names, ref_seqs, records, reads1, reads2=None, first_read_id=0):
     """SAM text from SAM cores (host only).  ref_seqs: list of uint8 arrays; reads*: (names, seqs, quals) lists of bytes."""
+    return _format_sam_host("cmx_format_sam", params, ref_names, ref_seqs, records, None, 0, reads1, reads2, first_read_id, None)
+
+
+def format_sam_bc(params, ref_names, ref_seqs, records, bcs, bc_len, reads1, reads2=None, first_read_id=0, translation=None):
+    """The same with cell barcodes (host only, cmx_format_sam_bc): bcs = one key per core (None: bulk), translation a
+    BarcodeTranslation or None.  Raises BarcodeNotTranslated, CmxError for the writer's other failures."""
+    return _format_sam_host("cmx_format_sam_bc", params, ref_names, ref_seqs, records, bcs, bc_len, reads1, reads2, first_read_id, translation)
+
+
+def _format_sam_host(fn, params, ref_names, ref_seqs, records, bcs, bc_len, reads1, reads2, first_read_id, translation):
     L = load_library()
     names = (C.c_char_p * len(ref_names))(*[s.encode() if isinstance(s, str) else s for s in ref_names])
     lens = np.array([len(s) for s in ref_seqs], dtype=np.uint32)
@@ -41,28 +65,25 @@ def format_sam(params, ref_names, ref_seqs, records, reads1, reads2=None, first_
     roff = np.zeros(len(ref_seqs) + 1, dtype=np.uint64)
     roff[1:] = np.cumsum(lens.astype(np.uint64))
     keep = []
-
-    def read_set(r):
-        if r is None:
-            return None
-        nm, sq, ql = r
-        arr = (C.c_char_p * len(nm))(*nm)
-        seq = np.frombuffer(b"".join(sq), dtype=np.uint8)
-        off = np.zeros(len(sq) + 1, dtype=np.uint64)
-        off[1:] = np.cumsum([len(x) for x in sq])
-        qual = np.frombuffer(b"".join(ql), dtype=np.uint8) if ql is not None else None
-        keep.extend([arr, seq, off, qual])
-        return ReadSet(C.cast(arr, C.c_void_p), seq.ctypes.data, off.ctypes.data, qual.ctypes.data if qual is not None else None)
-
-    r1, r2 = read_set(reads1), read_set(reads2)
+    r1, r2 = _sam_read_set(reads1, keep), _sam_read_set(reads2, keep)
     recs = np.ascontiguousarray(records)
-    args = (C.byref(params), names, lens.ctypes.data, len(ref_names), concat.ctypes.data, roff.ctypes.data, recs.ctypes.data, len(recs), C.byref(r1),
-            C.byref(r2) if r2 is not None else None, first_read_id)
-    n = L.cmx_format_sam(*args, None, 0)
+    head = (C.byref(params), names, lens.ctypes.data, len(ref_names), concat.ctypes.data, roff.ctypes.data, recs.ctypes.data)
+    reads = (C.byref(r1), C.byref(r2) if r2 is not None else None, first_read_id)
+    if fn == "cmx_format_sam":
+        args = head + (len(recs),) + reads
+    else:
+        bp = np.ascontiguousarray(bcs, dtype=np.uint64) if bcs is not None else None
+        t = translation.struct() if translation is not None else None
+        keep.extend([bp, t])
+        args = head + (bp.ctypes.data if bp is not None else None, bc_len, len(recs)) + reads + (C.byref(t) if t is not None else None,)
+    f = getattr(L, fn)
+    n = f(*args, None, 0)
+    if n == ERR_BARCODE_TRANSLATE:
+        raise BarcodeNotTranslated("Barcode does not exist in the translation table.")
     if n < 0:
-        raise CmxError("cmx_format_sam failed (%d)" % n)
+        raise CmxError("%s failed (%d)" % (fn, n))
     buf = C.create_string_buffer(n + 1)
-    assert L.cmx_format_sam(*args, buf, n) == n
+    assert f(*args, buf, n) == n
     return buf.raw[:n]
 
 
@@ -127,6 +148,9 @@ def apply_read_range(read_range, seq, qual=None):
 
 class _Translation(C.Structure):
     _fields_ = [("n", C.c_uint64), ("keys", C.c_void_p), ("to_off", C.c_void_p), ("to", C.c_void_p), ("from_len", C.c_uint32)]
+
+
+ERR_BARCODE_TRANSLATE = -8  # CMX_ERR_BARCODE_TRANSLATE
 
 
 class BarcodeNotTranslated(CmxError):
@@ -298,6 +322,11 @@ def load_library():
     L.cmx_format_paf.argtypes = [C.POINTER(Params), vp, vp, vp, u64, vp, vp, vp, vp, u32, vp, i64]
     L.cmx_format_sam.restype = i64
     L.cmx_format_sam.argtypes = [C.POINTER(Params), vp, vp, u32, vp, vp, vp, u64, C.POINTER(ReadSet), C.POINTER(ReadSet), u32, vp, i64]
+    L.cmx_format_sam_bc.restype = i64
+    L.cmx_format_sam_bc.argtypes = [C.POINTER(Params), vp, vp, u32, vp, vp, vp, vp, u32, u64, C.POINTER(ReadSet), C.POINTER(ReadSet), u32,
+                                    C.POINTER(_Translation), vp, i64]
+    L.cmx_format_sam_gpu.restype = i64
+    L.cmx_format_sam_gpu.argtypes = [vp, vp, vp, u32, vp, vp, u32, u64, C.POINTER(ReadSet), C.POINTER(ReadSet), u32, vp, i64]
     L.cmx_comm_unique_id.argtypes = [vp]
     L.cmx_comm_init.argtypes = [vp, i32, i32, vp]
     L.cmx_comm_destroy.argtypes = [vp]
@@ -399,12 +428,14 @@ class Mapper:
         offs[1:] = np.cumsum([len(s) for s in seqs])
         self._check(self.L.cmx_upload_reference(self.h, len(seqs), offs.ctypes.data, concat.ctypes.data), "cmx_upload_reference")
         self.names = names or ["chr%d" % (i + 1) for i in range(len(seqs))]
+        self.ref_lengths = np.diff(offs).astype(np.uint32)
 
     def upload_reference_ptr(self, ptr, offsets, names=None):
         """Reference already concatenated in (host or device) memory at `ptr`; offsets uint64[n_seq+1]."""
         offs = np.ascontiguousarray(offsets, dtype=np.uint64)
         self._check(self.L.cmx_upload_reference(self.h, len(offs) - 1, offs.ctypes.data, int(ptr)), "cmx_upload_reference")
         self.names = names or ["chr%d" % (i + 1) for i in range(len(offs) - 1)]
+        self.ref_lengths = np.diff(offs).astype(np.uint32)
 
     def upload_index(self, k, w, n_buckets, flags, keys, vals, occ):
         flags = np.ascontiguousarray(flags, dtype=np.uint32); keys = np.ascontiguousarray(keys, dtype=np.uint64)
@@ -682,6 +713,28 @@ class Mapper:
         buf = C.create_string_buffer(n + 1)
         m = self.L.cmx_format_bed_gpu(self.h, arr, recs.ctypes.data, bp, len(recs), bc_len, buf, n)
         assert m == n
+        return buf.raw[:n]
+
+    def format_sam_gpu(self, records, reads1, reads2=None, bcs=None, bc_len=0, first_read_id=0, ref_lengths=None, names=None):
+        """SAM text written on the device from SAM cores (bcs: one barcode key per core, None: bulk), with this context's
+        parameters and uploaded translation table; byte-identical to format_sam_bc.  reads*: (names, seqs, quals) lists of
+        bytes.  ref_lengths defaults to the uploaded sequences' lengths."""
+        names = names or self.names
+        arr = (C.c_char_p * len(names))(*[s.encode() for s in names])
+        lens = np.ascontiguousarray(ref_lengths if ref_lengths is not None else self.ref_lengths, dtype=np.uint32)
+        keep = []
+        r1, r2 = _sam_read_set(reads1, keep), _sam_read_set(reads2, keep)
+        recs = np.ascontiguousarray(records)
+        bp = np.ascontiguousarray(bcs, dtype=np.uint64) if bcs is not None else None
+        args = (self.h, arr, lens.ctypes.data, len(names), recs.ctypes.data, bp.ctypes.data if bp is not None else None, bc_len, len(recs), C.byref(r1),
+                C.byref(r2) if r2 is not None else None, first_read_id)
+        n = self.L.cmx_format_sam_gpu(*args, None, 0)
+        if n == ERR_BARCODE_TRANSLATE:
+            raise BarcodeNotTranslated(self.L.cmx_last_error(self.h).decode())
+        if n < 0:
+            raise CmxError("cmx_format_sam_gpu failed (%d): %s" % (n, self.L.cmx_last_error(self.h).decode()))
+        buf = C.create_string_buffer(n + 1)
+        assert self.L.cmx_format_sam_gpu(*args, buf, n) == n
         return buf.raw[:n]
 
     def format_tagalign(self, recs, names=None):

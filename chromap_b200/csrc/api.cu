@@ -15,11 +15,13 @@
 #include <string>
 #include <thread>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <thrust/iterator/counting_iterator.h>
+#include <thrust/iterator/transform_iterator.h>
 
 #include "../../include/chromap_b200.h"
 #include "cuda_owners.cuh"
@@ -32,6 +34,7 @@
 #include "allocate.cuh"
 #include "exchange.cuh"
 #include "sam_kernels.cuh"
+#include "sam_text.cuh"
 #include "ingest.cuh"
 #include "lane_pipeline.cuh"
 #include "host/read_range.h"
@@ -2185,6 +2188,171 @@ int64_t cmx_format_pairs_gpu(cmx_ctx *ctx, const char *const *names, const uint3
   if (buf && total <= cap) memcpy(buf, hdr.data(), hdr.size());
   if (n == 0) return total;
   return format_pairs_gpu(ctx, names, n_seq, records, n, read_names, n_read_names, first_read_id, buf, cap, &total) == CMX_OK ? total : -1;
+}
+
+struct WidenU64 {
+  __host__ __device__ u64 operator()(u32 x) const { return x; }
+};
+static_assert(std::is_same<std::iterator_traits<thrust::transform_iterator<WidenU64, const u32 *>>::value_type, u64>::value,
+              "SAM text offsets are scanned in 64 bits");
+// SAM text on the device (sam_text.cuh), byte-identical to cmx_format_sam_bc; the caller writes the @SQ header.  Cores, keys and
+// the reads of the call stay resident; lines are sorted by stable LSD radix passes over their ids, resolved, compacted, measured
+// and scanned over the whole call, then written in chunks of 1 M lines.  *text_err = -2 / -3 as the host twin returns them.
+static int format_sam_gpu(cmx_ctx *ctx, const char *const *ref_names, uint32_t n_seq, const cmx_sam_record *records, const uint64_t *barcode_keys,
+                          uint32_t bc_len, uint64_t n, const cmx_read_set *reads1, const cmx_read_set *reads2, uint32_t first_read_id, char *buf,
+                          int64_t cap, int64_t *total, int *text_err) {
+  if (!ctx->ref_seq || n_seq != ctx->n_seq) return fail(ctx, CMX_ERR_STATE, "cmx_format_sam_gpu: the reference of these names is not uploaded");
+  const bool pe = reads2 != nullptr;
+  const u64 n_lines = n * (pe ? 2 : 1);
+  if (n_lines > 0x7FFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "cmx_format_sam_gpu: more than 2^31-1 lines in one call");
+  cudaStream_t st = ctx->stream;
+  const unsigned nb = (unsigned)((n_lines + 255) / 256);
+  DevMem<OutSam> d_cores;
+  DevMem<u64> d_bc, d_k0, d_k1, d_small;
+  DevMem<u32> d_i0, d_i1, d_rnoff;
+  DevMem<u8> d_head, d_keep;
+  DevMem<char> d_rnames, d_out;
+  DevMem<> d_tmp;
+  CU(d_cores.alloc(n * sizeof(OutSam))); CU(d_small.alloc(64));
+  CU(cudaMemcpyAsync(d_cores, records, n * sizeof(OutSam), cudaMemcpyHostToDevice, st));
+  if (barcode_keys) { CU(d_bc.alloc(n * 8)); CU(cudaMemcpyAsync(d_bc, barcode_keys, n * 8, cudaMemcpyHostToDevice, st)); }
+  CU(d_k0.alloc((n_lines + 1) * 8)); CU(d_k1.alloc((n_lines + 1) * 8)); CU(d_i0.alloc(n_lines * 4)); CU(d_i1.alloc(n_lines * 4));
+  CU(d_head.alloc(n_lines)); CU(d_keep.alloc(n_lines));
+  // d_small: [0] largest key word 0, [1] err (overflowed cores, long CIGARs), [2] selected lines, [3] largest read index,
+  // [4, 5] missing translation segments / the first line that has one
+  CU(cudaMemsetAsync(d_small, 0, 64, st));
+  u64 *const max0 = d_small.p, *const nsel = d_small.p + 2;
+  int *const err = reinterpret_cast<int *>(d_small.p + 1);
+  u32 *const max_ri = reinterpret_cast<u32 *>(d_small.p + 3);
+  SamText T{};
+  T.cores = d_cores; T.bcs = barcode_keys ? d_bc.p : nullptr; T.pe = pe; T.bc_len = (int)bc_len; T.first_read_id = first_read_id;
+  T.ref = ctx->ref_seq; T.ref_off = ctx->ref_off;
+  sam_expand_kernel<<<nb, 256, 0, st>>>(T, n_lines, d_i0, max0, err);
+  sam_max_read_kernel<<<nb, 256, 0, st>>>(T, n_lines, max_ri);
+  u64 small[4];
+  CU(cudaMemcpyAsync(small, d_small, 32, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  if ((int)(small[1] & 0xFFFFFFFFu)) { *text_err = -2; return CMX_OK; }
+  const u64 n_reads = (u64)(u32)small[3] + 1;
+  if (n_reads > 0x7FFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "cmx_format_sam_gpu: a core's read id is below first_read_id");
+  // the reads of the call, and the reference names
+  DevMem<char> d_seq[2], d_qual[2], d_names[2];
+  DevMem<u64> d_off[2], d_noff[2];
+  std::string cat;
+  for (int mate = 0; mate < (pe ? 2 : 1); ++mate) {
+    const cmx_read_set &rs = mate ? *reads2 : *reads1;
+    if (!rs.names || !rs.seq || !rs.off) return fail(ctx, CMX_ERR_INVALID, "cmx_format_sam_gpu: read set without names, bases or offsets");
+    const u64 bytes = rs.off[n_reads];
+    std::vector<u64> noff(n_reads + 1, 0);
+    cat.clear();
+    for (u64 i = 0; i < n_reads; ++i) { cat += rs.names[i]; noff[i + 1] = cat.size(); }
+    CU(d_seq[mate].alloc(bytes + 1)); CU(d_off[mate].alloc((n_reads + 1) * 8)); CU(d_names[mate].alloc(cat.size() + 1)); CU(d_noff[mate].alloc((n_reads + 1) * 8));
+    CU(cudaMemcpyAsync(d_seq[mate], rs.seq, bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_off[mate], rs.off, (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_names[mate], cat.data(), cat.size(), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_noff[mate], noff.data(), (n_reads + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (rs.qual) { CU(d_qual[mate].alloc(bytes + 1)); CU(cudaMemcpyAsync(d_qual[mate], rs.qual, bytes, cudaMemcpyHostToDevice, st)); }
+    CU(cudaStreamSynchronize(st));  // (cat is reused)
+    T.r[mate] = SamReads{d_seq[mate], rs.qual ? d_qual[mate].p : nullptr, d_off[mate], d_names[mate], d_noff[mate]};
+  }
+  std::vector<u32> rnoff(n_seq + 1, 0);
+  cat.clear();
+  for (u32 i = 0; i < n_seq; ++i) { cat += ref_names[i]; rnoff[i + 1] = (u32)cat.size(); }
+  CU(d_rnames.alloc(cat.size() + 1)); CU(d_rnoff.alloc((n_seq + 1) * 4));
+  CU(cudaMemcpyAsync(d_rnames, cat.data(), cat.size(), cudaMemcpyHostToDevice, st)); CU(cudaMemcpyAsync(d_rnoff, rnoff.data(), (n_seq + 1) * 4, cudaMemcpyHostToDevice, st));
+  T.ref_names = d_rnames; T.ref_name_off = d_rnoff;
+  // order: least significant word first, every pass stable; the barcode word only for barcoded cores, the mate position only
+  // for paired-end ones (single-end lines all have 0)
+  cub::DoubleBuffer<u64> dk(d_k0, d_k1);
+  cub::DoubleBuffer<u32> di(d_i0, d_i1);
+  size_t tmp_bytes = 0, need = 0;
+  const int nl = (int)n_lines;
+  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, dk, di, nl, 0, 64, st);
+  cub::DeviceSelect::Flagged(nullptr, need, d_i0.p, d_keep.p, d_i1.p, nsel, nl, st);
+  tmp_bytes = std::max(tmp_bytes, need);
+  cub::DeviceScan::ExclusiveSum(nullptr, need, thrust::make_transform_iterator(static_cast<const u32 *>(d_i0.p), WidenU64()), d_k0.p, nl + 1, st);
+  tmp_bytes = std::max(tmp_bytes, need);
+  CU(d_tmp.alloc(tmp_bytes));
+  int bits0 = 1;
+  while (bits0 < 64 && (small[0] >> bits0)) ++bits0;
+  for (int w = 3; w >= 0; --w) {
+    if ((w == 1 && !barcode_keys) || (w == 2 && !pe)) continue;
+    sam_key_kernel<<<nb, 256, 0, st>>>(T, w, di.Current(), n_lines, dk.Current());
+    const int bits = w == 0 ? bits0 : w == 1 ? 2 * (int)bc_len : w == 2 ? 32 : 41;
+    CU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dk, di, nl, 0, bits, st));
+  }
+  const cmx_params &p = ctx->params;
+  u32 *const idx = di.Current(), *const res = di.Alternate();
+  sam_head_kernel<<<nb, 256, 0, st>>>(T, p.remove_pcr_duplicates, idx, n_lines, d_head);
+  sam_resolve_kernel<<<nb, 256, 0, st>>>(T, p.low_memory_mode, p.mapq_threshold, idx, d_head, n_lines, res, d_keep);
+  // the key buffers are free now: selected line ids and lengths in one, the text offsets in the other; NM over the ids
+  u32 *const sel = reinterpret_cast<u32 *>(dk.Alternate()), *const len = sel + n_lines, *const nm = idx;
+  u64 *const off = dk.Current();
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, res, d_keep.p, sel, nsel, nl, st));
+  CU(cudaMemcpyAsync(&small[2], nsel, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const u64 m = small[2];
+  BedTranslation Tr{};
+  const bool tr = barcode_keys && ctx->tr_n_slots;
+  unsigned long long *const miss = reinterpret_cast<unsigned long long *>(d_small.p + 4);
+  if (tr) {
+    const unsigned first_init = ~0u;
+    CU(cudaMemcpyAsync(d_small.p + 5, &first_init, 4, cudaMemcpyHostToDevice, st));
+    Tr.slots = ctx->tr_slots; Tr.mask = ctx->tr_n_slots - 1; Tr.shift = table_shift(ctx->tr_n_slots); Tr.from_len = (int)ctx->tr_from_len; Tr.to = ctx->tr_to;
+    Tr.n_missing = miss; Tr.first_missing = reinterpret_cast<unsigned *>(d_small.p + 5);
+  }
+  CU(cudaMemsetAsync(len + m, 0, 4, st));
+  if (m) sam_len_kernel<<<(unsigned)((m + 255) / 256), 256, 0, st>>>(T, sel, m, len, nm, err, Tr);
+  // the lengths are 32-bit, the text of a call is not: the scan must add in 64 bits (CUB's accumulator is the input's type)
+  CU(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, thrust::make_transform_iterator(static_cast<const u32 *>(len), WidenU64()), off, (int)m + 1, st));
+  u64 res_small[6];
+  CU(cudaMemcpyAsync(res_small, d_small, 48, cudaMemcpyDeviceToHost, st));
+  u64 bytes_all = 0;
+  CU(cudaMemcpyAsync(&bytes_all, off + m, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  if ((res_small[1] >> 32) != 0) { *text_err = -3; return CMX_OK; }
+  if (tr && res_small[4]) {
+    const u32 first_line = (u32)res_small[5];
+    u32 l = 0;
+    CU(cudaMemcpy(&l, sel + first_line, 4, cudaMemcpyDeviceToHost));
+    const u64 key = barcode_keys[pe ? l >> 1 : l];
+    std::string bc;
+    for (u32 j = 0; j < bc_len; ++j) bc += "ACGT"[(key >> ((bc_len - 1 - j) * 2)) & 3];
+    return fail(ctx, CMX_ERR_BARCODE_TRANSLATE, "%llu barcode segments have no entry in the translation table; the first is in barcode %s (SAM line %u)",
+                (unsigned long long)res_small[4], bc.c_str(), first_line);
+  }
+  const u64 CH = 1u << 20;
+  const bool fits = buf && *total + (int64_t)bytes_all <= cap;
+  for (u64 c0 = 0; fits && c0 < m; c0 += CH) {
+    const u64 k = std::min(CH, m - c0);
+    u64 ends[2];
+    CU(cudaMemcpyAsync(&ends[0], off + c0, 8, cudaMemcpyDeviceToHost, st)); CU(cudaMemcpyAsync(&ends[1], off + c0 + k, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const u64 bytes = ends[1] - ends[0];
+    if (bytes > d_out.cap) CU(d_out.alloc(bytes + bytes / 8));  // (alloc frees the smaller buffer first)
+    sam_write_kernel<<<(unsigned)((k * 32 + 255) / 256), 256, 0, st>>>(T, sel + c0, k, off + c0, ends[0], nm + c0, d_out, Tr);
+    CU(cudaMemcpyAsync(buf + *total + ends[0], d_out, bytes, cudaMemcpyDeviceToHost, st)); CU(cudaStreamSynchronize(st));
+  }
+  *total += (int64_t)bytes_all;
+  CU(cudaGetLastError());
+  return CMX_OK;
+}
+int64_t cmx_format_sam_gpu(cmx_ctx *ctx, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const cmx_sam_record *records,
+                           const uint64_t *barcode_keys, uint32_t bc_len, uint64_t n, const cmx_read_set *reads1, const cmx_read_set *reads2,
+                           uint32_t first_read_id, char *buf, int64_t cap) {
+  if (!ctx || !ref_names || !ref_lengths || (!records && n) || !reads1 || (barcode_keys && (bc_len == 0 || bc_len > 32))) return -1;
+  if (cudaSetDevice(ctx->device) != cudaSuccess) return -1;
+  std::string hdr;  // mapping_writer.cc:312-321
+  for (uint32_t i = 0; i < n_seq; ++i) hdr += std::string("@SQ\tSN:") + ref_names[i] + "\tLN:" + std::to_string(ref_lengths[i]) + "\n";
+  int64_t total = (int64_t)hdr.size();
+  if (buf && total <= cap) memcpy(buf, hdr.data(), hdr.size());
+  if (n == 0) return total;
+  int text_err = 0;
+  const int rc = format_sam_gpu(ctx, ref_names, n_seq, records, barcode_keys, bc_len, n, reads1, reads2, first_read_id, buf, cap, &total, &text_err);
+  if (rc == CMX_OK) return text_err ? text_err : total;
+  return rc == CMX_ERR_BARCODE_TRANSLATE ? rc : -1;
 }
 
 // --TagAlign for paired-end records (mapping_writer.cc:84-110): one line per mate, the duplicate count on the second.

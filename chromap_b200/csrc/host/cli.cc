@@ -396,8 +396,8 @@ static Options ParseOptions(int argc, char **argv) {
       printf("chromap-b200: chromap's paired-end BED path on H100 GPUs (subset of chromap options; see DESIGN.md)\n"
              "  --read-format STR   parts of read 1, read 2 and the barcode to keep, as chromap: comma-separated r1|r2|bc:start:end[:+|-]\n"
              "                      (0-based, inclusive, end -1 = the last base; ranges of one file ascending, '-' reverse-complements)\n"
-             "  --barcode-translate FILE  write barcoded BED fields through a TO,FROM (or TO<tab>FROM) table, plain or gzipped, as chromap\n"
-             "                      (e.g. ATAC to gene-expression barcodes of 10x Multiome); bulk runs ignore it\n"
+             "  --barcode-translate FILE  write barcoded BED fields and SAM CB:Z: tags through a TO,FROM (or TO<tab>FROM) table, plain or\n"
+             "                      gzipped, as chromap (e.g. ATAC to gene-expression barcodes of 10x Multiome); bulk runs ignore it\n"
              "  --bc-error-threshold INT  max Hamming distance allowed to correct a barcode against the whitelist: 0, 1 or 2 [1]\n"
              "  --bc-probability-threshold FLT  min probability of the best correction among the candidates [0.9]\n"
              "  --allocate-multi-mappings  give each multi-mapped read (MAPQ < 4) one of its mappings, drawn with weights = the\n"
@@ -454,7 +454,7 @@ static Options ParseOptions(int argc, char **argv) {
              a == "-p" || a == "--matrix-output-prefix")
       Die("chromap-b200: option " + a + " changes the output in ways that are not on the GPU path; use the reference chromap for it");
     else if (a == "--TagAlign") p.output_format = 2;  // same records as BED, TagAlign / PairedTagAlign text (chromap_driver.cc:417-418)
-    else if (a == "--SAM") p.output_format = 4;  // device: ksw spans, CIGARs, MAPQ; host: flags, NM / MD, order, text (cmx_format_sam)
+    else if (a == "--SAM") p.output_format = 4;  // device: ksw spans, CIGARs, MAPQ, then order, NM / MD and the text (cmx_format_sam_gpu)
     else if (a == "--PAF") o.paf = true;  // BED-path records, PAF text and order on the host (cmx_format_paf)
     else if (a == "--summary")
       Die("chromap-b200: option " + a + " is not on the GPU path yet (BED and Hi-C pairs only); use the reference chromap for it");
@@ -503,7 +503,7 @@ static void CheckMappingOptions(const Options &o) {
   if (o.index_path.empty()) Die("No index specified!");
   if (o.r1_path.empty()) Die("No read file specified!");
   if (o.se && o.pairs) Die("chromap-b200: pairs output needs paired-end reads");
-  if ((o.tagalign || o.sam || o.paf) && o.sc) Die("chromap-b200: --TagAlign / --SAM / --PAF with barcodes is not on the GPU path");
+  if ((o.tagalign || o.paf) && o.sc) Die("chromap-b200: --TagAlign / --PAF with barcodes is not on the GPU path");
   if (o.paf && (o.sam || o.tagalign || o.pairs || o.p.trim_adapters)) Die("chromap-b200: --PAF goes with BED-path mapping without adapter trimming (trimmed read lengths are not returned yet)");
   if (o.pairs && o.p.remove_pcr_duplicates && !o.p.low_memory_mode)  // RemovePCRDuplicate keeps the LAST record of a run (mapping_processor.h:181-197): not on the GPU path for pairs
     Die("chromap-b200: duplicate removal of Hi-C pairs needs --low-mem (or --preset hic)");
@@ -768,12 +768,19 @@ static void WriteOutput(const Options &o, uint32_t bc_len, Session *s, Mapped *m
   uint64_t keep = 0;
   std::vector<char> text;
   int64_t bytes = 0;
-  if (o.sam) {
+  if (o.sam) {  // bulk or barcoded (m->bc empty: bulk); the host twin without a table is exactly cmx_format_sam
     const cmx_read_set rs1{n1.data(), m->s1.data(), m->off1.data(), m->q1.data()}, rs2{n2.data(), m->s2.data(), m->off2.data(), m->q2.data()};
-    bytes = Format(&text, [&](char *buf, int64_t cap) { return cmx_format_sam(&o.p, names.data(), lens.data(), (uint32_t)names.size(), ref.concat.data(), ref.offsets.data(),
-                                                                              m->sam_cores.data(), m->sam_cores.size(), &rs1, o.se ? nullptr : &rs2, 0, buf, cap); });
-    if (bytes < 0) Die("chromap-b200: cmx_format_sam failed");
+    const uint64_t *bc = o.sc ? m->bc.data() : nullptr;
+    bytes = FormatOnDeviceElseHost(
+        ctx, &text,
+        [&](char *buf, int64_t cap) { return cmx_format_sam_gpu(ctx, names.data(), lens.data(), (uint32_t)names.size(), m->sam_cores.data(), bc, bc_len,
+                                                                m->sam_cores.size(), &rs1, o.se ? nullptr : &rs2, 0, buf, cap); },
+        [&](char *buf, int64_t cap) { return cmx_format_sam_bc(&o.p, names.data(), lens.data(), (uint32_t)names.size(), ref.concat.data(), ref.offsets.data(),
+                                                               m->sam_cores.data(), bc, bc_len, m->sam_cores.size(), &rs1, o.se ? nullptr : &rs2, 0,
+                                                               bc && !o.tr_path.empty() ? &s->tr : nullptr, buf, cap); });
+    if (bytes < 0) Die("chromap-b200: the SAM writer failed (" + std::to_string(bytes) + ")");
     keep = (uint64_t)std::count(text.begin(), text.begin() + bytes, '\n') - names.size();  // less the @SQ header
+    if (o.sc) fprintf(stderr, "Number of barcodes in whitelist: %llu.\nNumber of corrected barcodes: %llu.\n", (unsigned long long)m->n_bc_in, (unsigned long long)m->n_bc_cor);
   } else if (o.paf) {
     bytes = Format(&text, [&](char *buf, int64_t cap) { return cmx_format_paf(&o.p, names.data(), lens.data(), all.data(), all.size(), n1.data(), m->len1.data(),
                                                                               o.se ? nullptr : n2.data(), o.se ? nullptr : m->len2.data(), 0, buf, cap); });

@@ -1,12 +1,14 @@
 // chromap_b200 host side — SAM text from the device's SAM cores (cmx_sam_record): flags, mate fields and TLEN
 // (mapping_generator.h:613-640, mapping_generator.cc:84-107), NM / MD (alignment.cc:85-139), record order, duplicate
 // removal and MAPQ filter (sam_mapping.h:188-199, mapping_processor.h:161-202, mapping_writer.h:166-376, :405-437) and the
-// lines themselves (mapping_writer.cc:312-356).  No device needed.
+// lines themselves (mapping_writer.cc:312-356), with the cell barcode for barcoded runs.  No device needed; the device writes the
+// same text in sam_text.cuh, and this writer stays the specification it is tested against.
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <string>
 #include <tuple>
+#include <unordered_map>
 #include <vector>
 
 #include "../../../include/chromap_b200.h"
@@ -18,24 +20,31 @@ struct Line {
   int64_t pos, mpos;
   int rid, mrid, flag, tlen, mapq;
   uint32_t read_id;
+  uint64_t bc;  // cell barcode key (0: bulk)
 };
 inline int BaseCode(char c) {  // utils.h:87-104
   switch (c) { case 'A': case 'a': return 0; case 'C': case 'c': return 1; case 'G': case 'g': return 2; case 'T': case 't': return 3; default: return 4; }
 }
 }  // namespace
 
-extern "C" int64_t cmx_format_sam(const cmx_params *p, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const char *ref_concat,
-                                  const uint64_t *ref_offsets, const cmx_sam_record *records, uint64_t n, const cmx_read_set *reads1,
-                                  const cmx_read_set *reads2, uint32_t first_read_id, char *buf, int64_t cap) {
+// One writer for bulk and barcoded cores.  barcode_keys (NULL: bulk) is one key per core: it joins the order and the duplicate
+// test (sam_mapping.h:188-199) and is written as CB:Z: (mapping_writer.cc:350-354) through `tr` (NULL: the key's bases).
+static int64_t FormatSam(const cmx_params *p, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const char *ref_concat,
+                         const uint64_t *ref_offsets, const cmx_sam_record *records, const uint64_t *barcode_keys, uint32_t bc_len, uint64_t n,
+                         const cmx_read_set *reads1, const cmx_read_set *reads2, uint32_t first_read_id, const cmx_barcode_translation *tr, char *buf,
+                         int64_t cap) {
   if (!p || !ref_names || !ref_lengths || !ref_concat || !ref_offsets || (!records && n) || !reads1) return -1;
+  if (barcode_keys && (bc_len == 0 || bc_len > 32)) return -1;
+  if (barcode_keys && tr && (tr->from_len < 1 || tr->from_len > 31 || (tr->n && (!tr->keys || !tr->to_off)))) return -1;
   const bool pe = reads2 != nullptr;
   std::vector<Line> lines;
   lines.reserve(n * (pe ? 2 : 1));
   for (uint64_t i = 0; i < n; ++i) {
     const cmx_sam_record &c = records[i];
     if (c.overflow) return -2;
+    const uint64_t bc = barcode_keys ? barcode_keys[i] : 0;
     if (!pe) {
-      lines.push_back({&c, 0, (int64_t)c.pos[0], 0, (int)c.rid, -1, (c.strand[0] ? 0 : 16) | (c.secondary ? 256 : 0), 0, (int)c.mapq, c.read_id});
+      lines.push_back({&c, 0, (int64_t)c.pos[0], 0, (int)c.rid, -1, (c.strand[0] ? 0 : 16) | (c.secondary ? 256 : 0), 0, (int)c.mapq, c.read_id, bc});
       continue;
     }
     int f1 = 3 | 64, f2 = 3 | 128;
@@ -43,12 +52,14 @@ extern "C" int64_t cmx_format_sam(const cmx_params *p, const char *const *ref_na
     if (!c.strand[1]) { f1 |= 32; f2 |= 16; }
     if (c.secondary) { f1 |= 256; f2 |= 256; }
     const int tlen = c.strand[0] ? (int)(c.end[1] - c.pos[0] + 1u) : (int)(c.end[0] - c.pos[1] + 1u);  // PairedEndMappingInMemory::GetFragmentLength
-    lines.push_back({&c, 0, (int64_t)c.pos[0], (int64_t)c.pos[1], (int)c.rid, (int)c.rid, f1, c.strand[0] ? tlen : -tlen, (int)c.mapq, c.read_id});
-    lines.push_back({&c, 1, (int64_t)c.pos[1], (int64_t)c.pos[0], (int)c.rid, (int)c.rid, f2, c.strand[1] ? tlen : -tlen, (int)c.mapq, c.read_id});
+    lines.push_back({&c, 0, (int64_t)c.pos[0], (int64_t)c.pos[1], (int)c.rid, (int)c.rid, f1, c.strand[0] ? tlen : -tlen, (int)c.mapq, c.read_id, bc});
+    lines.push_back({&c, 1, (int64_t)c.pos[1], (int64_t)c.pos[0], (int)c.rid, (int)c.rid, f2, c.strand[1] ? tlen : -tlen, (int)c.mapq, c.read_id, bc});
   }
-  auto key = [](const Line &l) { return std::make_tuple(l.rid, l.pos, l.mrid, l.mpos, l.flag & 64, l.mapq, l.read_id); };
+  auto key = [](const Line &l) { return std::make_tuple(l.rid, l.pos, l.bc, l.mrid, l.mpos, l.flag & 64, l.mapq, l.read_id); };
   std::stable_sort(lines.begin(), lines.end(), [&](const Line &a, const Line &b) { return key(a) < key(b); });
-  auto same = [](const Line &a, const Line &b) { return a.rid == b.rid && a.pos == b.pos && (a.flag & 64) == (b.flag & 64) && a.mrid == b.mrid && a.mpos == b.mpos; };
+  auto same = [](const Line &a, const Line &b) {
+    return a.rid == b.rid && a.pos == b.pos && a.bc == b.bc && (a.flag & 64) == (b.flag & 64) && a.mrid == b.mrid && a.mpos == b.mpos;
+  };
   std::vector<const Line *> keep;
   if (p->remove_pcr_duplicates) {
     size_t i = 0;
@@ -57,10 +68,42 @@ extern "C" int64_t cmx_format_sam(const cmx_params *p, const char *const *ref_na
       for (; j < lines.size() && same(lines[j], lines[j - 1]); ++j) {
         if (p->low_memory_mode) { if (lines[j].mapq > lines[k].mapq) k = j; } else k = j;
       }
-      keep.push_back(&lines[k]);
+      if (lines[k].mapq >= p->mapq_threshold) keep.push_back(&lines[k]);
       i = j;
     }
-  } else for (const Line &l : lines) keep.push_back(&l);
+  } else for (const Line &l : lines) if (l.mapq >= p->mapq_threshold) keep.push_back(&l);
+  auto read_of = [&](const Line &l, const char **rseq, size_t *full, uint32_t *ri) {
+    const cmx_read_set &rs = l.mate == 0 ? *reads1 : *reads2;
+    *ri = l.core->read_id - first_read_id;
+    *rseq = rs.seq + rs.off[*ri];
+    *full = (size_t)(rs.off[*ri + 1] - rs.off[*ri]);
+    size_t rl = 0;  // the mapped read may be shorter than the record (adapter trimming keeps a prefix): its length is what the CIGAR consumes
+    for (int q = 0; q < l.core->n_cigar[l.mate]; ++q) if ((l.core->cigar[l.mate][q] & 0xf) != 2) rl += l.core->cigar[l.mate][q] >> 4;
+    return rl;
+  };
+  // the checks come before any text: a CIGAR longer than its read, then a barcode segment without a translation
+  for (const Line *l : keep) {
+    const char *rseq; size_t full; uint32_t ri;
+    if (read_of(*l, &rseq, &full, &ri) > full) return -3;
+  }
+  std::unordered_map<uint64_t, uint64_t> at;
+  if (barcode_keys && tr) for (uint64_t i = 0; i < tr->n; ++i) at[tr->keys[i]] = i;
+  auto cell_barcode = [&](uint64_t bc, std::string *out) {  // BarcodeTranslator::Translate (barcode_translator.h:72-123)
+    out->clear();
+    if (!tr) { for (uint32_t j = 0; j < bc_len; ++j) out->push_back("ACGT"[(bc >> ((bc_len - 1 - j) * 2)) & 3]); return true; }
+    const uint32_t L = tr->from_len, nseg = bc_len / L;
+    const uint64_t mask = (1ull << (2 * L)) - 1;
+    for (uint32_t s = 0; s < nseg; ++s) {
+      auto it = at.find((bc >> (2 * L * (nseg - 1 - s))) & mask);
+      if (it == at.end()) return false;
+      if (s) out->push_back('-');
+      out->append(tr->to + tr->to_off[it->second], tr->to_off[it->second + 1] - tr->to_off[it->second]);
+    }
+    return true;
+  };
+  std::string cb;
+  if (barcode_keys && tr)
+    for (const Line *l : keep) if (!cell_barcode(l->bc, &cb)) return CMX_ERR_BARCODE_TRANSLATE;
   int64_t len = 0;
   auto put = [&](const std::string &s) {
     if (buf && len + (int64_t)s.size() <= cap) memcpy(buf + len, s.data(), s.size());
@@ -69,16 +112,12 @@ extern "C" int64_t cmx_format_sam(const cmx_params *p, const char *const *ref_na
   for (uint32_t i = 0; i < n_seq; ++i) put(std::string("@SQ\tSN:") + ref_names[i] + "\tLN:" + std::to_string(ref_lengths[i]) + "\n");
   std::string seq, qual, cig, md, out;
   for (const Line *l : keep) {
-    if (l->mapq < p->mapq_threshold) continue;
     const cmx_sam_record &c = *l->core;
     const cmx_read_set &rs = l->mate == 0 ? *reads1 : *reads2;
-    const uint32_t ri = c.read_id - first_read_id;
-    const char *rseq = rs.seq + rs.off[ri];
-    const size_t full = (size_t)(rs.off[ri + 1] - rs.off[ri]);
-    // the mapped read may be shorter than the record (adapter trimming keeps a prefix): its length is what the CIGAR consumes
-    size_t rl = 0;
-    for (int q = 0; q < c.n_cigar[l->mate]; ++q) if ((c.cigar[l->mate][q] & 0xf) != 2) rl += c.cigar[l->mate][q] >> 4;
-    if (rl > full) return -3;
+    const char *rseq;
+    size_t full;
+    uint32_t ri;
+    const size_t rl = read_of(*l, &rseq, &full, &ri);
     const bool plus = c.strand[l->mate] != 0;
     if (plus) seq.assign(rseq, rl);
     else {  // PrepareNegativeSequenceAt on the kept prefix (sequence_batch.h:123-151)
@@ -111,10 +150,26 @@ extern "C" int64_t cmx_format_sam(const cmx_params *p, const char *const *ref_na
     out.assign(rs.names[ri]);
     out += "\t" + std::to_string(l->flag) + "\t" + ref_names[l->rid] + "\t" + std::to_string(l->pos + 1) + "\t" + std::to_string(l->mapq) + "\t" + cig + "\t";
     out += l->mrid < 0 ? "*" : (l->mrid == l->rid ? "=" : ref_names[l->mrid]);
-    out += "\t" + std::to_string(l->mrid < 0 ? 0 : l->mpos + 1) + "\t" + std::to_string(l->tlen) + "\t" + seq + "\t" + qual + "\tNM:i:" + std::to_string(nm) + "\tMD:Z:" + md + "\n";
+    out += "\t" + std::to_string(l->mrid < 0 ? 0 : l->mpos + 1) + "\t" + std::to_string(l->tlen) + "\t" + seq + "\t" + qual + "\tNM:i:" + std::to_string(nm) + "\tMD:Z:" + md;
+    if (barcode_keys) { cell_barcode(l->bc, &cb); out += "\tCB:Z:" + cb; }
+    out += "\n";
     put(out);
   }
   return len;
+}
+
+extern "C" int64_t cmx_format_sam(const cmx_params *p, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const char *ref_concat,
+                                  const uint64_t *ref_offsets, const cmx_sam_record *records, uint64_t n, const cmx_read_set *reads1,
+                                  const cmx_read_set *reads2, uint32_t first_read_id, char *buf, int64_t cap) {
+  return FormatSam(p, ref_names, ref_lengths, n_seq, ref_concat, ref_offsets, records, nullptr, 0, n, reads1, reads2, first_read_id, nullptr, buf, cap);
+}
+
+extern "C" int64_t cmx_format_sam_bc(const cmx_params *p, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const char *ref_concat,
+                                     const uint64_t *ref_offsets, const cmx_sam_record *records, const uint64_t *barcode_keys, uint32_t bc_len, uint64_t n,
+                                     const cmx_read_set *reads1, const cmx_read_set *reads2, uint32_t first_read_id,
+                                     const cmx_barcode_translation *translation, char *buf, int64_t cap) {
+  return FormatSam(p, ref_names, ref_lengths, n_seq, ref_concat, ref_offsets, records, barcode_keys, bc_len, n, reads1, reads2, first_read_id, translation, buf,
+                   cap);
 }
 
 // PAF text (mapping_writer.cc:177-196 single-end, :249-310 paired-end) from the BED-path records: PAFMapping /

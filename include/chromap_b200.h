@@ -373,6 +373,25 @@ typedef struct {
 int64_t cmx_format_sam(const cmx_params *p, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const char *ref_concat,
                        const uint64_t *ref_offsets, const cmx_sam_record *records, uint64_t n, const cmx_read_set *reads1,
                        const cmx_read_set *reads2, uint32_t first_read_id, char *buf, int64_t cap);
+/* The same for barcoded runs (host only): barcode_keys[i] (NULL: exactly cmx_format_sam) is the cell barcode key of core i, as
+ * cmx_map_batch_pe returns it; it joins the order (rid, pos, barcode, mrid, mpos, read 1, mapq, read id) and the duplicate
+ * test (pos, rid, barcode, read 1, mrid, mpos) of sam_mapping.h:188-199, and every line ends in "\tCB:Z:<field>"
+ * (mapping_writer.cc:350-354), the field being what cmx_format_bed_bc_tr writes for the key (translation NULL: its bc_len
+ * bases).  Returns -2 for an overflowed core, -3 for a CIGAR longer than its read, CMX_ERR_BARCODE_TRANSLATE with nothing
+ * written for a barcode segment without an entry in `translation`, -1 for bad arguments. */
+int64_t cmx_format_sam_bc(const cmx_params *p, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const char *ref_concat,
+                          const uint64_t *ref_offsets, const cmx_sam_record *records, const uint64_t *barcode_keys, uint32_t bc_len, uint64_t n,
+                          const cmx_read_set *reads1, const cmx_read_set *reads2, uint32_t first_read_id,
+                          const cmx_barcode_translation *translation, char *buf, int64_t cap);
+/* The SAM text written on the device, byte-identical to cmx_format_sam_bc (barcode_keys NULL: cmx_format_sam) with the
+ * context's parameters (duplicate rule, MAPQ threshold) and, for barcoded cores, the translation table of
+ * cmx_upload_barcode_translation.  NM / MD are computed against the uploaded reference.  Host buffers in and out; the @SQ
+ * header is written by the host.  Cores, keys, reads and the sort's scratch are resident on the device for the call (232 B per
+ * core + 26 B per line + the reads' bases, qualities and names + 16 B per read; see DESIGN.md): a call that does not fit returns
+ * -1, as does any other device failure.  -2, -3 and CMX_ERR_BARCODE_TRANSLATE as the host twin.  buf == NULL returns the length. */
+int64_t cmx_format_sam_gpu(cmx_ctx *ctx, const char *const *ref_names, const uint32_t *ref_lengths, uint32_t n_seq, const cmx_sam_record *records,
+                           const uint64_t *barcode_keys, uint32_t bc_len, uint64_t n, const cmx_read_set *reads1, const cmx_read_set *reads2,
+                           uint32_t first_read_id, char *buf, int64_t cap);
 
 /* --PAF (MAPPINGFORMAT_PAF = 3) text from the BED-path records (host only): PAFMapping / PairedPAFMapping hold the same
  * fields plus read names and the (trimmed) read lengths; order, duplicate rule, Tn5 shift and MAPQ filter are those types'
