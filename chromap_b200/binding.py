@@ -210,6 +210,27 @@ def format_bed_bc_tr(names, recs, bcs, bc_len, translation):
     return buf.raw[:n]
 
 
+class BulkDedupError(CmxError):
+    """A bulk-level duplicate removal refused: its status in `.status` (records untouched)."""
+
+    def __init__(self, msg, status):
+        super().__init__(msg)
+        self.status = status
+
+
+def postprocess_bc_bulk(params, wl_keys, wl_counts, recs, bcs):
+    """Host twin of Mapper.postprocess_bc_bulk_gpu (the reference's low-memory merge loop at bulk level), with the whitelist
+    given as keys and their counts.  Returns (records, barcode keys); raises BulkDedupError."""
+    L = load_library()
+    recs = np.ascontiguousarray(recs.copy()); bcs = np.ascontiguousarray(np.array(bcs, dtype=np.uint64).copy())
+    wk = np.ascontiguousarray(wl_keys, dtype=np.uint64); wc = np.ascontiguousarray(wl_counts, dtype=np.uint32)
+    n = C.c_uint64()
+    rc = L.cmx_postprocess_bc_bulk(C.byref(params), wk.ctypes.data, wc.ctypes.data, len(wk), recs.ctypes.data, bcs.ctypes.data, len(recs), C.byref(n))
+    if rc != 0:
+        raise BulkDedupError("cmx_postprocess_bc_bulk failed (%d)" % rc, rc)
+    return recs[:n.value], bcs[:n.value]
+
+
 class Batch(C.Structure):
     _fields_ = [("n_pairs", C.c_uint32), ("seq1", C.c_void_p), ("off1", C.c_void_p), ("seq2", C.c_void_p),
                 ("off2", C.c_void_p), ("first_read_id", C.c_uint32), ("on_device", C.c_int32),
@@ -342,6 +363,8 @@ def load_library():
     L.cmx_upload_barcode_translation.argtypes = [vp, C.POINTER(_Translation)]
     L.cmx_format_bed_bc_tr.restype = i64; L.cmx_format_bed_bc_tr.argtypes = [vp, vp, vp, u64, u32, C.POINTER(_Translation), vp, i64]
     L.cmx_ingest_fastq_range.argtypes = [vp, i32, vp, u64, i32, vp, C.POINTER(ReadRange), C.POINTER(Ingested)]
+    L.cmx_postprocess_bc_bulk_gpu.argtypes = [vp, vp, vp, u64, C.POINTER(u64)]
+    L.cmx_postprocess_bc_bulk.argtypes = [C.POINTER(Params), vp, vp, u64, vp, vp, u64, C.POINTER(u64)]
     for f in (L.cmx_allocate_multi_mappings_gpu, L.cmx_allocate_multi_mappings):
         f.argtypes = [vp, vp, vp, u64, C.c_int32, C.c_int32, C.POINTER(u64), C.POINTER(AllocationStats)]
     _lib = L
@@ -627,6 +650,16 @@ class Mapper:
         self._check(self.L.cmx_postprocess_gpu(self.h, recs.ctypes.data, bcs.ctypes.data if bcs is not None else None, len(recs), C.byref(n)),
                     "cmx_postprocess_gpu")
         return recs[:n.value] if bcs is None else (recs[:n.value], bcs[:n.value])
+
+    def postprocess_bc_bulk_gpu(self, recs, bcs):
+        """Barcoded records de-duplicated at bulk level on the device, with the uploaded whitelist's abundances (low-memory
+        context that removes duplicates).  Returns (records, barcode keys); raises BulkDedupError with the status."""
+        recs = np.ascontiguousarray(recs.copy()); bcs = np.ascontiguousarray(np.array(bcs, dtype=np.uint64).copy())
+        n = C.c_uint64()
+        rc = self.L.cmx_postprocess_bc_bulk_gpu(self.h, recs.ctypes.data, bcs.ctypes.data, len(recs), C.byref(n))
+        if rc != 0:
+            raise BulkDedupError("cmx_postprocess_bc_bulk_gpu failed (%d): %s" % (rc, self.L.cmx_last_error(self.h).decode()), rc)
+        return recs[:n.value], bcs[:n.value]
 
     def _allocate(self, fn, what, recs, bcs, distance, seed):
         recs = np.ascontiguousarray(recs.copy())

@@ -16,6 +16,7 @@
 #include <thread>
 #include <tuple>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -1425,7 +1426,51 @@ int64_t cmx_format_bed_bc(const char *const *names, const cmx_pe_record *recs, c
 // Sort + duplicate removal + MAPQ filter (+ Tn5 shift) over device-resident records: d_a[0, n) (and d_bca) in, the result in
 // d_b[0, *nsel) (and d_bcb); d_a is used as scratch.  All four buffers hold n entries.  Work is queued on ctx->stream and
 // waited for.
-static int pp_device(cmx_ctx *ctx, const PpParams &P, PpRecord *d_a, u64 *d_bca, u64 n, PpRecord *d_b, u64 *d_bcb, u64 *nsel_out) {
+struct MaxU64 {
+  __device__ u64 operator()(u64 a, u64 b) const { return a > b ? a : b; }
+};
+static size_t pp_bulk_tmp_bytes(u64 n, cudaStream_t st) {  // CUB scratch of pp_bulk_resolve
+  size_t a = 0, b = 0;
+  cub::DeviceScan::InclusiveSum(nullptr, a, (const u32 *)nullptr, (u32 *)nullptr, (int)n, st);
+  cub::DeviceReduce::ReduceByKey(nullptr, b, (const u32 *)nullptr, (u32 *)nullptr, (const u64 *)nullptr, (u64 *)nullptr, (u32 *)nullptr, MaxU64(), (int)n, st);
+  return std::max(a, b);
+}
+// Bulk-level duplicate removal (postprocess.cuh, pp_bulk_*) of the sorted barcoded records recs / bcs [0, n): one candidate per
+// bulk group in res / res_bc [0, *n_groups), keep_flag set by the MAPQ filter.  k0, k1 (n u64), i0, i1 (n u32) and tmp
+// (pp_bulk_tmp_bytes) are scratch.  CMX_ERR_INVALID for a barcode that is not in the whitelist.
+static int pp_bulk_resolve(cmx_ctx *ctx, const PpParams &P, const PpAbundance &wl, const PpRecord *recs, const u64 *bcs, u64 n, u64 *k0, u64 *k1, u32 *i0, u32 *i1,
+                           DevMem<> &tmp, PpRecord *res, u64 *res_bc, u8 *keep_flag, u64 *n_groups_out) {
+  cudaStream_t st = ctx->stream;
+  const unsigned nb = (unsigned)((n + 255) / 256);
+  DevMem<u32> d_small;  // [0] groups, [1] highest MAPQ of the last group, [2..3] barcodes missing from the whitelist (u64)
+  CU(d_small.alloc(16));
+  CU(cudaMemsetAsync(d_small, 0, 16, st));
+  PpAbundance A = wl;
+  A.n_missing = (unsigned long long *)(d_small.p + 2);
+  pp_bulk_entry_kernel<<<nb, 256, 0, st>>>(P.se, recs, bcs, n, A, i0, k0);
+  size_t tmp_bytes = tmp.cap;
+  CU(cub::DeviceScan::InclusiveSum(tmp.p, tmp_bytes, i0, i1, (int)n, st));  // i1 = 1-based group of each record
+  tmp_bytes = tmp.cap;
+  CU(cub::DeviceReduce::ReduceByKey(tmp.p, tmp_bytes, i1, i0, k0, k1, d_small.p, MaxU64(), (int)n, st));  // k1[g] = best key of group g
+  u32 small[4] = {0, 0, 0, 0};
+  CU(cudaMemcpyAsync(small, d_small, 16, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  CU(cudaGetLastError());
+  const u32 n_groups = small[0];
+  const u64 n_missing = (u64)small[2] | ((u64)small[3] << 32);
+  if (n_missing)
+    return fail(ctx, CMX_ERR_INVALID, "bulk-level duplicate removal: %llu barcode(s) of the records are not in the whitelist, whose abundance the rule needs",
+                (unsigned long long)n_missing);
+  pp_bulk_heads_kernel<<<nb, 256, 0, st>>>(i1, n, i0);  // i0[g] = first record of group g
+  pp_bulk_last_mapq_kernel<<<nb, 256, 0, st>>>(recs, i0, n_groups, n, d_small.p + 1);
+  pp_bulk_resolve_kernel<<<(n_groups + 255) / 256, 256, 0, st>>>(P, recs, bcs, k1, i0, n_groups, n, d_small.p + 1, res, res_bc, keep_flag);
+  CU(cudaGetLastError());
+  *n_groups_out = n_groups;
+  return CMX_OK;
+}
+
+static int pp_device(cmx_ctx *ctx, const PpParams &P, PpRecord *d_a, u64 *d_bca, u64 n, PpRecord *d_b, u64 *d_bcb, u64 *nsel_out,
+                     const PpAbundance *wl = nullptr) {
   *nsel_out = 0;
   if (n == 0) return CMX_OK;
   if (n > 0x7FFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "post-processing: more than 2^31-1 records in one call");
@@ -1448,6 +1493,7 @@ static int pp_device(cmx_ctx *ctx, const PpParams &P, PpRecord *d_a, u64 *d_bca,
   tmp_bytes = std::max(tmp_bytes, need);
   cub::DeviceSelect::Flagged(nullptr, need, d_bca, d_keep.p, d_bcb, d_nsel.p, (int)n, st);
   tmp_bytes = std::max(tmp_bytes, need);
+  if (P.bulk) tmp_bytes = std::max(tmp_bytes, pp_bulk_tmp_bytes(n, st));
   CU(d_tmp.alloc(tmp_bytes));
   // only the bits a key word can hold are sorted: word 0 (rid | start, or rid1 | rid2) up to its largest value in this call;
   // pp_key_word bounds the others: the 32-bit alignment lengths; length alone; mapq | direction | unique | read id
@@ -1468,10 +1514,16 @@ static int pp_device(cmx_ctx *ctx, const PpParams &P, PpRecord *d_a, u64 *d_bca,
     CU(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, dk, di, (int)n, 0, bits, st));
   }
   pp_gather_kernel<<<nb, 256, 0, st>>>(d_a, bc ? d_bca : nullptr, di.Current(), n, d_b, d_bcb);
-  pp_head_kernel<<<nb, 256, 0, st>>>(P.kind, P.se, P.dedup, d_b, bc ? d_bcb : nullptr, n, d_head);
-  pp_resolve_kernel<<<nb, 256, 0, st>>>(P, d_b, bc ? d_bcb : nullptr, d_head, n, d_a, bc ? d_bca : nullptr, d_keep);
-  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_a, d_keep.p, d_b, d_nsel.p, (int)n, st));
-  if (bc) CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_bca, d_keep.p, d_bcb, d_nsel + 1, (int)n, st));
+  u64 n_res = n;  // entries of d_a / d_keep the compaction reads: one per record, or one per bulk group
+  if (P.bulk) {
+    const int rc = pp_bulk_resolve(ctx, P, *wl, d_b, d_bcb, n, d_k0, d_k1, d_i0, d_i1, d_tmp, d_a, d_bca, d_keep, &n_res);
+    if (rc != CMX_OK) return rc;
+  } else {
+    pp_head_kernel<<<nb, 256, 0, st>>>(P.kind, P.se, P.dedup, d_b, bc ? d_bcb : nullptr, n, d_head);
+    pp_resolve_kernel<<<nb, 256, 0, st>>>(P, d_b, bc ? d_bcb : nullptr, d_head, n, d_a, bc ? d_bca : nullptr, d_keep);
+  }
+  CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_a, d_keep.p, d_b, d_nsel.p, (int)n_res, st));
+  if (bc) CU(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_bca, d_keep.p, d_bcb, d_nsel + 1, (int)n_res, st));
   u64 nsel = 0;
   CU(cudaMemcpyAsync(&nsel, d_nsel, 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
@@ -1507,6 +1559,120 @@ int cmx_postprocess_gpu(cmx_ctx *ctx, void *records, uint64_t *barcode_keys, uin
   if (rc != CMX_OK) return rc;
   if (nsel) CU(cudaMemcpyAsync(records, d_b, nsel * sizeof(PpRecord), cudaMemcpyDeviceToHost, st));
   if (bc && nsel) CU(cudaMemcpyAsync(barcode_keys, d_bcb, nsel * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  *n_out = nsel;
+  return CMX_OK;
+}
+
+// ---- --remove-pcr-duplicates-at-bulk-level for barcoded BED (mapping_writer.h:126-163, 166-376) ------------------------------
+// Why a context cannot take the rule, or nullptr
+static const char *bulk_dedup_refusal(const cmx_params &p) {
+  if (!p.low_memory_mode) return "only the low-memory merge has bulk-level duplicate removal (in memory the reference removes duplicates per cell)";
+  if (!p.remove_pcr_duplicates) return "the context does not remove duplicates";
+  if (p.output_format == 4 || p.output_format == 5) return "bulk-level duplicate removal covers BED records, not SAM or pairs";
+  return nullptr;
+}
+// The merge loop of ProcessAndOutputMappingsInLowMemory, one record at a time, over the records in the reference's order
+static int postprocess_bc_bulk_host(const cmx_params &p, const std::unordered_map<uint64_t, uint32_t> &abundance, cmx_pe_record *recs, uint64_t *bcs,
+                                    uint64_t n, uint64_t *n_out) {
+  *n_out = 0;
+  if (n == 0) return CMX_OK;
+  std::vector<uint64_t> ord(n);
+  for (uint64_t i = 0; i < n; ++i) ord[i] = i;
+  auto key = [&](uint64_t i) {  // bed_mapping.h:32-37,145-153 prefixed by rid
+    const cmx_pe_record &r = recs[i];
+    return std::make_tuple(r.rid, r.fragment_start, r.fragment_length, bcs[i], r.mapq, r.direction, r.is_unique, r.read_id);
+  };
+  std::stable_sort(ord.begin(), ord.end(), [&](uint64_t a, uint64_t b) { return key(a) < key(b); });
+  for (uint64_t i = 0; i < n; ++i)
+    if (!abundance.count(bcs[i])) return CMX_ERR_INVALID;
+  const bool se = p.single_end != 0;
+  auto same_position = [&](uint64_t a, uint64_t b) {  // IsSamePosition, bed_mapping.h:43-45,155-158
+    return recs[a].fragment_start == recs[b].fragment_start && (se || recs[a].fragment_length == recs[b].fragment_length);
+  };
+  auto same = [&](uint64_t a, uint64_t b) { return bcs[a] == bcs[b] && same_position(a, b); };  // operator==, bed_mapping.h:39-42,159-163
+  struct Entry { uint64_t rec; uint32_t num_dups; };
+  std::vector<Entry> entries;
+  auto best = [&]() {  // FindBestMappingIndexFromDuplicates
+    size_t b = 0;
+    for (size_t k = 1; k < entries.size(); ++k) {
+      const uint32_t ab = abundance.at(bcs[entries[k].rec]), bb = abundance.at(bcs[entries[b].rec]);
+      if (entries[k].num_dups > entries[b].num_dups || (entries[k].num_dups == entries[b].num_dups && ab > bb)) b = k;
+    }
+    return entries[b].rec;
+  };
+  std::vector<cmx_pe_record> out_r;
+  std::vector<uint64_t> out_b;
+  auto emit = [&](uint64_t i, uint32_t dups) {
+    cmx_pe_record r = recs[i];
+    r.num_dups = (uint8_t)std::min<uint32_t>(255, dups);
+    if (p.tn5_shift) { if (se) tn5_se(r); else tn5(r); }
+    out_r.push_back(r); out_b.push_back(bcs[i]);
+  };
+  uint64_t last = 0;
+  uint32_t num_last_dups = 0;
+  for (uint64_t k = 0; k < n; ++k) {
+    const uint64_t cur = ord[k];
+    const bool duplicated = k > 0 && recs[cur].rid == recs[last].rid && (same(cur, last) || same_position(cur, last));
+    if (duplicated) {
+      ++num_last_dups;
+      if (!entries.empty() && same(cur, entries.back().rec)) entries.back() = Entry{cur, 2};
+      else entries.push_back(Entry{cur, 1});
+      if (recs[cur].mapq > recs[last].mapq) last = cur;
+    } else {
+      if (k > 0) {
+        last = best();
+        entries.clear();
+        if (recs[last].mapq >= p.mapq_threshold) emit(last, num_last_dups);
+      }
+      last = cur;
+      num_last_dups = 1;
+      entries.push_back(Entry{cur, 1});
+    }
+  }
+  if (recs[last].mapq >= p.mapq_threshold) emit(best(), num_last_dups);  // the last group: tested before its best entry is chosen
+  std::copy(out_r.begin(), out_r.end(), recs);
+  std::copy(out_b.begin(), out_b.end(), bcs);
+  *n_out = out_r.size();
+  return CMX_OK;
+}
+
+int cmx_postprocess_bc_bulk(const cmx_params *p, const uint64_t *wl_keys, const uint32_t *wl_counts, uint64_t n_wl, cmx_pe_record *records,
+                            uint64_t *barcode_keys, uint64_t n, uint64_t *n_out) {
+  if (!p || (n_wl && (!wl_keys || !wl_counts)) || (n && (!records || !barcode_keys)) || !n_out) return CMX_ERR_INVALID;
+  if (bulk_dedup_refusal(*p) || n > 0x7FFFFFFFull) return CMX_ERR_INVALID;
+  if (n_wl == 0) return CMX_ERR_STATE;
+  std::unordered_map<uint64_t, uint32_t> abundance;
+  for (uint64_t i = 0; i < n_wl; ++i) abundance.emplace(wl_keys[i], wl_counts[i]);
+  return postprocess_bc_bulk_host(*p, abundance, records, barcode_keys, n, n_out);
+}
+
+int cmx_postprocess_bc_bulk_gpu(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_keys, uint64_t n, uint64_t *n_out) {
+  if (!ctx || (n && (!records || !barcode_keys)) || !n_out) return CMX_ERR_INVALID;
+  const cmx_params &p = ctx->params;
+  if (const char *why = bulk_dedup_refusal(p)) return fail(ctx, CMX_ERR_INVALID, "cmx_postprocess_bc_bulk_gpu: %s", why);
+  if (!ctx->wl_active) return fail(ctx, CMX_ERR_STATE, "cmx_postprocess_bc_bulk_gpu: no barcode whitelist uploaded; the rule ranks barcodes by their abundance in it");
+  if (ctx->wl_output_nw)
+    return fail(ctx, CMX_ERR_INVALID, "cmx_postprocess_bc_bulk_gpu: barcodes outside the whitelist (output_not_in_whitelist) have no abundance; the reference reads past its table for them");
+  if (n > 0x7FFFFFFFull) return fail(ctx, CMX_ERR_INVALID, "cmx_postprocess_bc_bulk_gpu: more than 2^31-1 records in one call");
+  *n_out = 0;
+  if (n == 0) return CMX_OK;
+  CU(cudaSetDevice(ctx->device));
+  PpParams P;
+  P.kind = PP_BED_BC; P.low_mem = 1; P.dedup = 1; P.tn5 = p.tn5_shift; P.mapq_threshold = p.mapq_threshold; P.se = p.single_end; P.bulk = 1;
+  const PpAbundance wl{ctx->wl_slots, ctx->wl_n_slots - 1, table_shift(ctx->wl_n_slots), nullptr};
+  cudaStream_t st = ctx->stream;
+  DevMem<PpRecord> d_a, d_b;
+  DevMem<u64> d_bca, d_bcb;
+  CU(d_a.alloc(n * sizeof(PpRecord))); CU(d_b.alloc(n * sizeof(PpRecord)));
+  CU(d_bca.alloc(n * 8)); CU(d_bcb.alloc(n * 8));
+  CU(cudaMemcpyAsync(d_a, records, n * sizeof(PpRecord), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_bca, barcode_keys, n * 8, cudaMemcpyHostToDevice, st));
+  u64 nsel = 0;
+  const int rc = pp_device(ctx, P, d_a, d_bca, n, d_b, d_bcb, &nsel, &wl);
+  if (rc != CMX_OK) return rc;
+  if (nsel) CU(cudaMemcpyAsync(records, d_b, nsel * sizeof(PpRecord), cudaMemcpyDeviceToHost, st));
+  if (nsel) CU(cudaMemcpyAsync(barcode_keys, d_bcb, nsel * 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   *n_out = nsel;
   return CMX_OK;

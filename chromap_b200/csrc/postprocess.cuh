@@ -8,6 +8,7 @@
 // words (CUB SortPairs is stable); the record index is the payload, records are gathered once at the end.
 #pragma once
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -21,6 +22,7 @@ struct PpRecord {  // 24 bytes, viewed as cmx_pe_record or cmx_pairs_record
 
 struct PpParams {
   int kind, low_mem, dedup, tn5, mapq_threshold, se;
+  int bulk = 0;  // PP_BED_BC with the low-memory rule: duplicates removed at bulk level (pp_bulk_* kernels)
 };
 
 // cmx_pe_record: w0 read_id, w1 rid, w2 fragment_start, w3 = fragment_length | mapq<<16 | direction<<24,
@@ -137,6 +139,76 @@ __global__ void pp_resolve_kernel(PpParams P, const PpRecord *recs, const u64 *b
     if (res_bc) res_bc[i] = keep_bc;
   }
   keep_flag[i] = k;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Bulk-level duplicate removal of barcoded records (mapping_writer.h:126-163, 166-376), in place of pp_head_kernel and
+// pp_resolve_kernel on the sorted records.  A bulk group is a run of records at the same position (rid, start, and length when
+// paired-end); an entry is a run of consecutive records of one barcode inside a group.  An entry stands for its last record and
+// weighs 1 (one record) or 2 (more: the merge overwrites the stored record, whose num_dups_ is 1, then adds 1).  A group keeps
+// the record of its first entry with the greatest (weight, barcode abundance) and counts its records as duplicates.  No thread
+// walks a group (scATAC hot spots hold 10^5 records and more): each entry tail gets a key whose maximum over the group, taken
+// by CUB's reduce-by-key, names the survivor.
+struct PpAbundance {  // the whitelist (cmx_upload_barcode_whitelist): barcode key -> count among the sampled barcodes
+  const ulonglong2 *slots;
+  u64 mask;
+  int shift;
+  unsigned long long *n_missing;  // += entries whose barcode is not in the table
+};
+__device__ __forceinline__ bool pp_same_position(int se, const PpRecord &a, const PpRecord &b) {  // IsSamePosition, bed_mapping.h:43-45,155-158
+  return a.w[1] == b.w[1] && a.w[2] == b.w[2] && (se || pe_len(a) == pe_len(b));
+}
+// head[i] = 1 at the first record of a bulk group.  key[i] = 0 inside an entry; at its last record
+// (weight - 1) << 63 | abundance << 31 | (0x7FFFFFFF - i): the greatest key of a group is its first best entry (n < 2^31).
+__global__ void pp_bulk_entry_kernel(int se, const PpRecord *recs, const u64 *bcs, u64 n, PpAbundance A, u32 *head, u64 *key) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const PpRecord r = recs[i];
+  const u64 bc = bcs[i];
+  const bool group_head = i == 0 || !pp_same_position(se, recs[i - 1], r);
+  const bool entry_head = group_head || bcs[i - 1] != bc;
+  const bool entry_tail = i + 1 == n || !pp_same_position(se, r, recs[i + 1]) || bcs[i + 1] != bc;
+  head[i] = group_head ? 1u : 0u;
+  u64 k = 0;
+  if (entry_tail) {
+    u64 abundance = 0;
+    if (!kv_find(A.slots, A.mask, A.shift, bc, &abundance)) atomicAdd(A.n_missing, 1ull);
+    k = ((u64)!entry_head << 63) | ((abundance & 0xFFFFFFFFull) << 31) | (0x7FFFFFFFull - i);
+  }
+  key[i] = k;
+}
+// group_pos[g] = the first record of group g (gid = 1-based group of each record, the inclusive scan of head)
+__global__ void pp_bulk_heads_kernel(const u32 *gid, u64 n, u32 *group_pos) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && (i == 0 || gid[i] != gid[i - 1])) group_pos[gid[i] - 1] = (u32)i;
+}
+// *mapq = the highest MAPQ of the last group: the merge tests the last group's threshold on it (mapping_writer.h:323-337).
+// Only records followed by a lower MAPQ (or by nothing) can hold it; inside a group they end runs of one length and barcode.
+__global__ void pp_bulk_last_mapq_kernel(const PpRecord *recs, const u32 *group_pos, u32 n_groups, u64 n, unsigned *mapq) {
+  const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || i < group_pos[n_groups - 1]) return;
+  const u32 mq = pe_mapq(recs[i]);
+  if (i + 1 < n && pe_mapq(recs[i + 1]) >= mq) return;
+  atomicMax(mapq, mq);
+}
+// One thread per group: its best entry's record with num_dups = min(255, group size), the MAPQ filter (the last group's on
+// *last_mapq), Tn5.  Out of place (recs -> res[g]).
+__global__ void pp_bulk_resolve_kernel(PpParams P, const PpRecord *recs, const u64 *bcs, const u64 *best, const u32 *group_pos, u32 n_groups, u64 n,
+                                       const unsigned *last_mapq, PpRecord *res, u64 *res_bc, u8 *keep_flag) {
+  const u64 g = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_groups) return;
+  const u32 b = 0x7FFFFFFFu - (u32)(best[g] & 0x7FFFFFFFull);
+  const u32 dups = (u32)((g + 1 < n_groups ? (u64)group_pos[g + 1] : n) - group_pos[g]);
+  PpRecord keep = recs[b];
+  const u32 mq = g + 1 == n_groups ? *last_mapq : pe_mapq(keep);
+  const bool k = (int)mq >= P.mapq_threshold;
+  if (k) {
+    keep.w[4] = (keep.w[4] & 0xFFFF00FFu) | ((dups > 255u ? 255u : dups) << 8);
+    if (P.tn5) pp_tn5_any(P.kind, P.se, keep);
+    res[g] = keep;
+    res_bc[g] = bcs[b];
+  }
+  keep_flag[g] = k;
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -195,6 +195,21 @@ int cmx_postprocess_bc(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_k
  * same way; results are identical to the host routines.  n < 2^31 per call. */
 int cmx_postprocess_gpu(cmx_ctx *ctx, void *records, uint64_t *barcode_keys, uint64_t n, uint64_t *n_out);
 
+/* --remove-pcr-duplicates-at-bulk-level for barcoded BED in a low-memory run (mapping_writer.h:126-163, 166-376), the reference's
+ * default for single-cell data: records at one position (rid, start, and length when paired-end) form one bulk group whatever
+ * their barcodes.  Within a group, each run of consecutive records of one barcode is an entry that stands for its last record
+ * and weighs 1 (one record) or 2 (more).  The group keeps the record of its first entry with the greatest (weight, abundance of
+ * its barcode in the whitelist), with num_dups = min(255, group size), if that record's MAPQ passes the threshold; the last
+ * group is tested on its highest MAPQ instead.  Tn5 follows.  In place on host buffers like cmx_postprocess_gpu, with the
+ * abundances of the uploaded whitelist.  CMX_ERR_STATE without a whitelist; CMX_ERR_INVALID for a context that is not
+ * low-memory, does not remove duplicates, emits SAM or pairs or outputs barcodes outside the whitelist, for n >= 2^31 and for a
+ * barcode missing from the whitelist.  Records are untouched in every refused case. */
+int cmx_postprocess_bc_bulk_gpu(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *barcode_keys, uint64_t n, uint64_t *n_out);
+/* Host twin (the reference's merge loop, one record at a time), needing no device: the whitelist is passed as n_wl keys and
+ * their counts.  The same results and refusals, CMX_ERR_STATE when n_wl == 0. */
+int cmx_postprocess_bc_bulk(const cmx_params *p, const uint64_t *wl_keys, const uint32_t *wl_counts, uint64_t n_wl, cmx_pe_record *records,
+                            uint64_t *barcode_keys, uint64_t n, uint64_t *n_out);
+
 /* --allocate-multi-mappings: counts of one call (the reference's log lines, mapping_processor.h:363,431-435,502-504). */
 typedef struct {
   uint64_t n_multi;            /* multi-mappings (mapq < 4) after duplicate removal: "Got all X multi-mappings!" */
