@@ -107,6 +107,8 @@ struct cmx_ctx {
   DevMem<double> wl_pow;
   u32 wl_bc_len = 0;
   int wl_err = 1, wl_output_nw = 0, wl_active = 0;
+  int wl_top_listed = 0;  // the key ~0 (all-T 32-mer) is listed with count wl_top_count: wl_lookup answers for it
+  u64 wl_top_count = 0;
   double wl_prob = 0.9;
   DevBuf bc_seq, bc_qual;
   // --barcode-translate table (cmx_upload_barcode_translation); tr_n_slots == 0: none
@@ -414,6 +416,10 @@ int cmx_upload_barcode_whitelist(cmx_ctx *ctx, const uint64_t *keys, const uint3
   CU(cudaSetDevice(ctx->device));
   // the old whitelist goes before the new one is allocated; a failed upload leaves none
   ctx->wl_slots.reset(); ctx->wl_n_slots = 0; ctx->wl_active = 0;
+  int top_listed = 0;
+  u64 top_count = 0;
+  for (u64 i = 0; i < n; ++i)
+    if (keys[i] == CMX_EMPTY_KEY) { top_listed = 1; top_count = counts[i]; }
   u64 ns = 64;
   while (ns < 2 * n) ns <<= 1;
   DevMem<ulonglong2> slots;
@@ -437,7 +443,7 @@ int cmx_upload_barcode_whitelist(cmx_ctx *ctx, const uint64_t *keys, const uint3
     ctx->wl_pow = std::move(d_pow);
   }
   ctx->wl_slots = std::move(slots); ctx->wl_n_slots = ns; ctx->wl_num_sample = num_sample; ctx->wl_bc_len = bc_len; ctx->wl_err = err_threshold; ctx->wl_prob = prob_threshold;
-  ctx->wl_output_nw = output_not_in_whitelist; ctx->wl_active = 1;
+  ctx->wl_output_nw = output_not_in_whitelist; ctx->wl_top_listed = top_listed; ctx->wl_top_count = top_count; ctx->wl_active = 1;
   return CMX_OK;
 }
 
@@ -699,7 +705,7 @@ struct LaneOnDevice {
 static cudaError_t dev_whitelist(const cmx_ctx *ctx, Lane &L, u32 n, DevWhitelist *W) {
   W->slots = ctx->wl_slots; W->mask = ctx->wl_n_slots ? ctx->wl_n_slots - 1 : 0; W->shift = ctx->wl_n_slots ? table_shift(ctx->wl_n_slots) : 0;
   W->num_sample = (double)ctx->wl_num_sample; W->pow_tab = ctx->wl_pow; W->err_threshold = ctx->wl_err; W->prob_threshold = ctx->wl_prob;
-  W->output_not_in_whitelist = ctx->wl_output_nw; W->active = ctx->wl_active;
+  W->output_not_in_whitelist = ctx->wl_output_nw; W->active = ctx->wl_active; W->top_listed = ctx->wl_top_listed; W->top_count = ctx->wl_top_count;
   W->c2_list = W->c2_over = nullptr; W->c2_slab = nullptr;
   if (!ctx->wl_active || ctx->wl_err != 2) return cudaSuccess;
   cudaError_t e = ensure(L.bc2_list, (size_t)n * 4);
@@ -1660,7 +1666,7 @@ int cmx_postprocess_bc_bulk_gpu(cmx_ctx *ctx, cmx_pe_record *records, uint64_t *
   CU(cudaSetDevice(ctx->device));
   PpParams P;
   P.kind = PP_BED_BC; P.low_mem = 1; P.dedup = 1; P.tn5 = p.tn5_shift; P.mapq_threshold = p.mapq_threshold; P.se = p.single_end; P.bulk = 1;
-  const PpAbundance wl{ctx->wl_slots, ctx->wl_n_slots - 1, table_shift(ctx->wl_n_slots), nullptr};
+  const PpAbundance wl{ctx->wl_slots, ctx->wl_n_slots - 1, table_shift(ctx->wl_n_slots), nullptr, ctx->wl_top_listed, ctx->wl_top_count};
   cudaStream_t st = ctx->stream;
   DevMem<PpRecord> d_a, d_b;
   DevMem<u64> d_bca, d_bcb;

@@ -231,6 +231,13 @@ __device__ __forceinline__ bool kv_find(const ulonglong2 *slots, u64 mask, int s
     s = (s + 1) & mask;
   }
 }
+// kv_find for the whitelist, whose keys take all 64 bits: the all-T 32-base barcode's key is CMX_EMPTY_KEY itself.  That key
+// never enters the slots (wl_insert_kernel skips it); top_listed and top_count, set by cmx_upload_barcode_whitelist, answer
+// for it.  The --barcode-translate table needs no such care: its FROM keys have at most 31 bases, so they stay below ~0.
+__device__ __forceinline__ bool wl_lookup(const ulonglong2 *slots, u64 mask, int shift, int top_listed, u64 top_count, u64 key, u64 *count) {
+  if (key == CMX_EMPTY_KEY) { *count = top_count; return top_listed != 0; }
+  return kv_find(slots, mask, shift, key, count);
+}
 // The slot that holds `key`, claimed for it if the key is new (concurrent inserts of other keys are safe).
 __device__ __forceinline__ ulonglong2 *kv_claim(ulonglong2 *slots, u64 mask, int shift, u64 key) {
   u64 s = (key * 0x9E3779B97F4A7C15ull) >> shift;

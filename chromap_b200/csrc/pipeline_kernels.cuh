@@ -2187,6 +2187,8 @@ struct DevWhitelist {
   const ulonglong2 *slots;  // {key, count}; empty key = ~0
   u64 mask;                 // n_slots - 1
   int shift;
+  int top_listed;           // the key ~0 (all-T at 32 bases) is listed, with count top_count: it cannot be in the slots
+  u64 top_count;
   double num_sample;
   const double *pow_tab;    // [81]: pow(10.0, (-q) / 10.0) from the host libm (q up to 40 + 40: two changed bases)
   int err_threshold;
@@ -2198,10 +2200,10 @@ struct DevWhitelist {
   u32 *c2_list, *c2_over;
   Bc2Slab *c2_slab;
 };
-__device__ __forceinline__ bool wl_find(const DevWhitelist &W, u64 key, u64 *count) { return kv_find(W.slots, W.mask, W.shift, key, count); }
+__device__ __forceinline__ bool wl_find(const DevWhitelist &W, u64 key, u64 *count) { return wl_lookup(W.slots, W.mask, W.shift, W.top_listed, W.top_count, key, count); }
 __global__ void wl_insert_kernel(const u64 *keys, const u32 *counts, u64 n, ulonglong2 *slots, u64 mask, int shift) {
   const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  if (i >= n || keys[i] == CMX_EMPTY_KEY) return;  // DevWhitelist::top_listed holds that one
   ulonglong2 *slot = kv_claim(slots, mask, shift, keys[i]);
   slot->y = counts[i];
 }

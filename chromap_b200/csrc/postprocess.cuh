@@ -154,6 +154,8 @@ struct PpAbundance {  // the whitelist (cmx_upload_barcode_whitelist): barcode k
   u64 mask;
   int shift;
   unsigned long long *n_missing;  // += entries whose barcode is not in the table
+  int top_listed;                 // the key ~0, kept out of the slots (wl_lookup)
+  u64 top_count;
 };
 __device__ __forceinline__ bool pp_same_position(int se, const PpRecord &a, const PpRecord &b) {  // IsSamePosition, bed_mapping.h:43-45,155-158
   return a.w[1] == b.w[1] && a.w[2] == b.w[2] && (se || pe_len(a) == pe_len(b));
@@ -172,7 +174,7 @@ __global__ void pp_bulk_entry_kernel(int se, const PpRecord *recs, const u64 *bc
   u64 k = 0;
   if (entry_tail) {
     u64 abundance = 0;
-    if (!kv_find(A.slots, A.mask, A.shift, bc, &abundance)) atomicAdd(A.n_missing, 1ull);
+    if (!wl_lookup(A.slots, A.mask, A.shift, A.top_listed, A.top_count, bc, &abundance)) atomicAdd(A.n_missing, 1ull);
     k = ((u64)!entry_head << 63) | ((abundance & 0xFFFFFFFFull) << 31) | (0x7FFFFFFFull - i);
   }
   key[i] = k;
@@ -256,7 +258,7 @@ __device__ __forceinline__ u32 bed_barcode_field(const BedTranslation &T, u64 bc
   u32 l = 0;
   for (int s = 0; s < nseg; ++s) {
     if (s) { if (p) p[l] = '-'; ++l; }
-    u64 v;
+    u64 v;  // a FROM key has at most 31 bases, so it is never CMX_EMPTY_KEY (wl_lookup's case)
     if (!kv_find(T.slots, T.mask, T.shift, (bc >> (2 * L * (nseg - 1 - s))) & seg_mask, &v)) { ++*n_missing; continue; }
     const u32 tl = (u32)(v & 0xFFFFu);
     if (p) { const char *t = T.to + (v >> 16); for (u32 k = 0; k < tl; ++k) p[l + k] = t[k]; }
