@@ -337,6 +337,7 @@ def load_library():
     L.cmx_last_batch_trace.argtypes = [vp, vp, u32]
     L.cmx_last_batch_timing.argtypes = [vp, C.POINTER(Timing)]
     L.cmx_set_lanes.argtypes = [vp, i32]
+    L.cmx_set_max_read_length.argtypes = [vp, i32]
     L.cmx_host_register.argtypes = [vp, u64]
     L.cmx_host_unregister.argtypes = [vp]
     L.cmx_format_paf.restype = i64
@@ -624,6 +625,10 @@ class Mapper:
 
     def set_lanes(self, n):
         self._check(self.L.cmx_set_lanes(self.h, int(n)), "cmx_set_lanes")
+
+    def set_max_read_length(self, n):
+        """Resize the context for reads of up to n bases (cmx_set_max_read_length)."""
+        self._check(self.L.cmx_set_max_read_length(self.h, int(n)), "cmx_set_max_read_length")
 
     def timing(self):
         t = Timing()

@@ -159,6 +159,38 @@ static int fail(cmx_ctx *c, int code, const char *fmt, ...) {
 
 static cudaError_t ensure(DevBuf &b, size_t bytes) { return bytes <= b.cap ? cudaSuccess : b.alloc(bytes + bytes / 8 + 256); }
 
+// A kernel's dynamic shared-memory limit is one setting per process, shared by every context: it is only ever raised, so
+// that a context sized for shorter reads never lowers it under one sized for longer reads.
+template <typename K>
+static cudaError_t raise_smem_limit(K *kernel, size_t bytes) {
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaFuncGetAttributes(&fa, kernel);
+  if (e == cudaSuccess && (size_t)fa.maxDynamicSharedSizeBytes < bytes) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  return e;
+}
+// Everything sized by the longest read a context maps (cmx_create, cmx_set_max_read_length): the shared memory of the
+// kernels that stage a whole read per thread or per tile or tier 0's hits per thread, the front end's persistent grid, and every lane's tier
+// capacities.  The lanes' scratch must hold no tier laid out for other capacities (it is regrown from the new ones).
+static cudaError_t size_for_read_length(cmx_ctx *ctx, int mrl) {
+  cudaError_t e = cudaSuccess;
+  if ((size_t)2 * mrl * 64 > 48 * 1024) e = raise_smem_limit(verify_kernel, (size_t)2 * mrl * 64);  // per-thread read-code columns (long reads)
+  if (e == cudaSuccess) e = raise_smem_limit(cluster_kernel, (size_t)tier0_hits(mrl) * CLUSTER_NT * 8);  // tier 0's hit rows
+  const size_t sf_smem = seed_front_smem_bytes(mrl);
+  if (e == cudaSuccess) e = raise_smem_limit(seed_front_kernel<true>, sf_smem);
+  if (e == cudaSuccess) e = raise_smem_limit(seed_front_kernel<false>, sf_smem);
+  int per_sm = 0, n_sm = 0;
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, seed_front_kernel<true>, SF_NT, sf_smem);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, ctx->device);
+  if (e != cudaSuccess) return e;
+  ctx->sf_grid = std::max(1, per_sm) * std::max(1, n_sm);
+  ctx->params.max_read_length = mrl;
+  for (Lane &L : ctx->lanes)
+    for (int t = 0; t < N_TIERS; ++t) L.tiers[t].caps = tier_caps(mrl, t);
+  return cudaSuccess;
+}
+// the verification kernels' read-code columns (2 x 64 x max_read_length bytes of shared memory per CTA) bound the length
+static const int MAX_READ_LENGTH_LIMIT = 1600;
+
 extern "C" {
 
 void cmx_default_params(cmx_params *p) {
@@ -188,10 +220,10 @@ int cmx_create(cmx_ctx **out, int device, const cmx_params *params) {
   if (!(((params->output_format == 1 || params->output_format == 2 || params->output_format == 4) && !params->split_alignment) ||
         (params->output_format == 5 && params->split_alignment)))
     return CMX_ERR_INVALID;  // BED / TagAlign (same records), SAM cores, or Hi-C pairs with split alignment
-  if (params->output_format == 4 && (params->max_read_length > SAM_MAX_L || params->error_threshold > SAM_MAX_E)) return CMX_ERR_INVALID;
+  if (params->output_format == 4 && (params->max_read_length > SAM_MAX_L_LONG || params->error_threshold > SAM_MAX_E)) return CMX_ERR_INVALID;
   if (params->error_threshold < 1 || params->error_threshold >= 16) return CMX_ERR_INVALID;  // mapping_parameters.h:80-88
   if (params->max_num_best_mappings < 1 || params->max_num_best_mappings > CMX_MAX_BEST) return CMX_ERR_INVALID;
-  if (params->batch_size < 1 || params->max_read_length < params->min_read_length) return CMX_ERR_INVALID;
+  if (params->batch_size < 1 || params->max_read_length < params->min_read_length || params->max_read_length > MAX_READ_LENGTH_LIMIT) return CMX_ERR_INVALID;
   if (params->single_end && (params->split_alignment || params->output_format == 5)) return CMX_ERR_INVALID;  // single-end: BED / TagAlign only
   if (params->output_format == 5 && params->remove_pcr_duplicates && !params->low_memory_mode) return CMX_ERR_INVALID;  // pairs dedup: low-memory rule only
   std::unique_ptr<cmx_ctx> owner(new cmx_ctx);  // an early return deletes the partial context
@@ -238,22 +270,7 @@ int cmx_create(cmx_ctx **out, int device, const cmx_params *params) {
   CU(cudaFuncSetAttribute(verify_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   CU(cudaFuncSetAttribute(pairing_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   CU(cudaFuncSetAttribute(verify_split_cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  const int mrl = params->max_read_length;
-  if ((size_t)2 * mrl * 64 > 48 * 1024) {  // per-thread read-code columns of the verification kernels (long reads)
-    if ((size_t)2 * mrl * 64 > 200 * 1024) return CMX_ERR_INVALID;
-    CU(cudaFuncSetAttribute(verify_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * mrl * 64));
-  }
-  {
-    const size_t sf_smem = seed_front_smem_bytes(mrl);
-    CU(cudaFuncSetAttribute(seed_front_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sf_smem));
-    CU(cudaFuncSetAttribute(seed_front_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sf_smem));
-    int per_sm = 0, n_sm = 0;
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, seed_front_kernel<true>, SF_NT, sf_smem));
-    CU(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
-    ctx->sf_grid = std::max(1, per_sm) * std::max(1, n_sm);
-  }
-  for (Lane &L : ctx->lanes)
-    for (int t = 0; t < N_TIERS; ++t) L.tiers[t].caps = tier_caps(mrl, t);
+  CU(size_for_read_length(ctx, params->max_read_length));
   memset(&ctx->timing, 0, sizeof(ctx->timing));
   *out = owner.release();
   return CMX_OK;
@@ -1060,6 +1077,26 @@ int cmx_set_lanes(cmx_ctx *ctx, int n_lanes) {
       for (Tier &t : L.tiers) { t.mem.reset(); t.ovf_list.reset(); t.slots_cap = 0; }
   }
   ctx->n_lanes = n_lanes;
+  return CMX_OK;
+}
+
+int cmx_set_max_read_length(cmx_ctx *ctx, int32_t L) {
+  if (!ctx) return CMX_ERR_INVALID;
+  const cmx_params &p = ctx->params;
+  if (L < p.min_read_length || L > MAX_READ_LENGTH_LIMIT || (p.output_format == 4 && L > SAM_MAX_L_LONG))
+    return fail(ctx, CMX_ERR_INVALID, "max_read_length %d: use %d .. %d%s", (int)L, p.min_read_length, p.output_format == 4 ? SAM_MAX_L_LONG : MAX_READ_LENGTH_LIMIT,
+                p.output_format == 4 ? " with SAM output" : "");
+  CU(cudaSetDevice(ctx->device));
+  int smem_optin = 0;
+  CU(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+  if (seed_front_smem_bytes(L) > (size_t)smem_optin)  // 64 reads per front-end tile: up to 843 bases in an H100's 227 KB
+    return fail(ctx, CMX_ERR_INVALID, "max_read_length %d: the front end's read tiles need %zu bytes of shared memory, the device has %d", (int)L,
+                seed_front_smem_bytes(L), smem_optin);
+  CU(cudaDeviceSynchronize());
+  // every tier's scratch was laid out for the old capacities: released here, regrown by the next call (as cmx_set_lanes does)
+  for (Lane &Ln : ctx->lanes)
+    for (Tier &t : Ln.tiers) { t.mem.reset(); t.ovf_list.reset(); t.slots_cap = 0; }
+  CU(size_for_read_length(ctx, L));
   return CMX_OK;
 }
 

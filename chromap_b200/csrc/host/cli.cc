@@ -67,9 +67,10 @@ struct Batch {
   std::string q1, q2;               // qualities in the layout of s1 / s2 (SAM only)
   std::string bc, bq;               // cell barcodes + qualities, bc_len bytes per pair (scATAC)
   uint32_t n = 0;
+  uint32_t max_len = 0;  // the longest read of either mate
   bool dev = false;      // reads were packed on the device (cmx_ingest_fastq): dev_in holds device pointers
   cmx_batch dev_in{};
-  void Clear() { dev = false; s1.clear(); s2.clear(); o1.assign(1, 0); o2.assign(1, 0); names1.clear(); names2.clear(); q1.clear(); q2.clear(); bc.clear(); bq.clear(); n = 0; }
+  void Clear() { dev = false; s1.clear(); s2.clear(); o1.assign(1, 0); o2.assign(1, 0); names1.clear(); names2.clear(); q1.clear(); q2.clear(); bc.clear(); bq.clear(); n = 0; max_len = 0; }
 };
 
 // Raw text of one read file for the device-side FASTQ parser.  Plain files are read with read(2) straight into a page-locked
@@ -302,7 +303,7 @@ static bool LoadBatchGpu(cmx_ctx *ctx, RawFile *f1, RawFile *f2, RawFile *fb, in
   if (f2) f2->Consume(c2);
   if (fb) fb->Consume(cb);
   g_t_fill += Now() - t_c0;
-  b->n = n1; b->dev = true;
+  b->n = n1; b->dev = true; b->max_len = std::max(g1.max_len, f2 ? g2.max_len : 0u);
   b->dev_in.n_pairs = n1; b->dev_in.seq1 = g1.seq; b->dev_in.off1 = g1.off; b->dev_in.on_device = 1;
   if (f2) { b->dev_in.seq2 = g2.seq; b->dev_in.off2 = g2.off; }
   if (fb) { b->dev_in.bc_seq = gb.seq; b->dev_in.bc_qual = gb.qual; b->dev_in.bc_len = bc_len; }
@@ -362,6 +363,8 @@ static uint32_t LoadBatch(SeqReader &r1, SeqReader &r2, uint32_t max_pairs, Batc
     if (!a && !c && !d) break;
     if (a != c || c != d) Die("Numbers of reads and barcodes don't match!");
     ++b->n;
+    b->max_len = std::max(b->max_len, b->o1[b->n] - b->o1[b->n - 1]);
+    if (!se) b->max_len = std::max(b->max_len, b->o2[b->n] - b->o2[b->n - 1]);
   }
   if (n_short || n_empty)
     DieReadRange(rf, std::to_string(n_short) + " reads end before a range of the read format does, " + std::to_string(n_empty) + " reads are empty after the cut");
@@ -402,6 +405,8 @@ static Options ParseOptions(int argc, char **argv) {
     else if (a == "-i" || a == "--build-index") o.build_index = true;
     else if (a == "-h" || a == "--help") {
       printf("chromap-b200: chromap's paired-end BED path on H100 GPUs (subset of chromap options; see DESIGN.md)\n"
+             "                      Reads of any length up to 832 bases map at full size: the mapping scratch grows to the longest read\n"
+             "                      (--SAM: reads of up to 320 bases; a longer read stops the run before any output is written)\n"
              "  -1, -2, -b FILE     read 1, read 2 and cell barcode files: one path, a comma-separated list, or quoted glob patterns\n"
              "                      (e.g. -1 'L00*_R1.fq.gz'; each pattern's matches sorted, the lists in argument order).  File i of -1\n"
              "                      goes with file i of -2 and -b; each file starts new batches of 500,000 reads, as chromap\n"
@@ -793,6 +798,48 @@ static size_t PlainFileBytes(const std::vector<std::string> &paths) {
   }
   return total;
 }
+// Reads longer than the context is sized for (cmx_params.max_read_length, 160 bases unless resized): before the call that
+// holds them maps, the context grows to the call's longest read rounded up to a multiple of 32 bases (at most 832: the front
+// end stages 64 reads per tile in shared memory, 227 KB on an H100; longer reads go to the overflow tiers).  Otherwise every
+// such pair would take an overflow tier, sized for the few pairs a genome sends there.  SAM aligns reads of up to 320 bases: a longer read ends the run here, before any output file is written.
+static void SizeForReads(const Options &o, cmx_ctx *ctx, uint32_t max_len, int32_t *L) {
+  if ((int64_t)max_len <= *L) return;
+  if (o.sam && max_len > 320)
+    Die("chromap-b200: --SAM on the GPU path aligns reads of up to 320 bases, and a read of " + std::to_string(max_len) + " bases was found; no output file is written");
+  const int32_t want = (int32_t)std::min<uint32_t>((max_len + 31) / 32 * 32, o.sam ? 320u : 832u);
+  if (want <= *L) return;  // already at the largest size: the longer reads take the overflow tiers
+  if (cmx_set_max_read_length(ctx, want)) Die(cmx_last_error(ctx));
+  fprintf(stderr, "Reads of up to %u bases: mapping scratch resized for %d-base reads.\n", max_len, want);
+  *L = want;
+}
+// Reference batches one library call maps at once.  Above 160 bases a call maps one batch at a time: a pair's tier-0
+// scratch grows with the read length, and so does the share of pairs that reach the overflow tiers, which hold each such pair
+// in megabytes (tier 2: about 3.5 MB).  On bench.py's 3 Gbp genome 0.48 % of 2x150 pairs reach tier 2 at 160 bases and
+// 0.84 % of 2x250 pairs at 256 (DESIGN.md §9).  Batches stay whole, so the output does not change.
+static uint32_t BatchesPerCall(int32_t L) { return L <= 160 ? 4u : 1u; }
+// One loaded call through the library, BatchesPerCall(L) reference batches at a time; records and counters summed into *out.
+static void MapCall(const Options &o, cmx_ctx *ctx, int32_t L, const cmx_batch &in, cmx_records *out, cmx_sam_record *sam_out) {
+  const uint32_t step = BatchesPerCall(L) * (uint32_t)o.p.batch_size;
+  cmx_records sum = *out;
+  for (uint32_t p0 = 0; p0 < in.n_pairs; p0 += step) {
+    cmx_batch part = in;
+    part.n_pairs = std::min(step, in.n_pairs - p0);
+    part.first_read_id += p0;
+    part.off1 += p0;
+    if (part.off2) part.off2 += p0;
+    if (part.bc_seq) { part.bc_seq += (size_t)p0 * in.bc_len; part.bc_qual += (size_t)p0 * in.bc_len; }
+    cmx_records r = *out;
+    r.records = sam_out ? reinterpret_cast<cmx_pe_record *>(sam_out + sum.n_records) : out->records + sum.n_records;
+    r.capacity = out->capacity - sum.n_records;
+    if (out->barcode_keys) r.barcode_keys = out->barcode_keys + sum.n_records;
+    if (cmx_map_batch_pe(ctx, &part, &r, nullptr)) Die(cmx_last_error(ctx));
+    if (p0 == 0) { sum = r; sum.records = out->records; sum.capacity = out->capacity; sum.barcode_keys = out->barcode_keys; continue; }
+    sum.n_records += r.n_records; sum.n_mapped_pairs += r.n_mapped_pairs; sum.n_uniquely_mapped_pairs += r.n_uniquely_mapped_pairs;
+    sum.n_candidates += r.n_candidates; sum.n_overflow_pairs += r.n_overflow_pairs;
+    sum.n_barcodes_in_whitelist += r.n_barcodes_in_whitelist; sum.n_barcodes_corrected += r.n_barcodes_corrected;
+  }
+  *out = sum;
+}
 // double-buffered batch loop: the loader thread prepares call c+1 while the GPU maps call c (chromap.h:871-877), opening the
 // next file set when the current one ends, so a file switch overlaps the mapping of the set's last call.
 static void MapReads(const Options &o, uint32_t bc_len, Session *s, Mapped *m) {
@@ -809,6 +856,7 @@ static void MapReads(const Options &o, uint32_t bc_len, Session *s, Mapped *m) {
   int n_calls = 0;
   std::vector<cmx_sam_record> sam_recs;
   std::vector<uint64_t> bc_keys;
+  int32_t read_len = o.p.max_read_length;  // what the context is sized for
   if (!s->gpu_reader) sets.Load(&cur, parity);
   while (cur.n > 0) {
     parity ^= 1;
@@ -833,8 +881,9 @@ static void MapReads(const Options &o, uint32_t bc_len, Session *s, Mapped *m) {
     out.records = recs.data(); out.capacity = recs.size();
     if (o.sam) { sam_recs.resize(recs.size()); out.records = reinterpret_cast<cmx_pe_record *>(sam_recs.data()); }
     if (o.sc) { bc_keys.resize(recs.size()); out.barcode_keys = bc_keys.data(); }
+    SizeForReads(o, ctx, cur.max_len, &read_len);
     const double t0 = Now();
-    if (cmx_map_batch_pe(ctx, &in, &out, nullptr)) Die(cmx_last_error(ctx));
+    MapCall(o, ctx, read_len, in, &out, o.sam ? sam_recs.data() : nullptr);
     fprintf(stderr, o.se ? "Mapped %u reads in %.2fs.\n" : "Mapped %u read pairs in %.2fs.\n", cur.n, Now() - t0);
     t_calls += Now() - t0; ++n_calls;
     const double t_col0 = Now();

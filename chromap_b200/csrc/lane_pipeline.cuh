@@ -40,10 +40,16 @@ inline DevParams dev_params(const Params &p, int k, int w) {
   return d;
 }
 
+// Tier 0's hit capacity: 64, and above 160 bases as many hits per base as at 160 (a read has about 2L / (w + 1) minimizers,
+// each with one hit or more), in whole cluster-kernel rows of 16, at most TIER0_HC_MAX: cluster_kernel holds a read's hits
+// in shared memory, hc x CLUSTER_NT x 8 bytes per CTA (192 KB at the cap).
+#define TIER0_HC_MAX 192
+inline int tier0_hits(int max_read_length) { return std::min(TIER0_HC_MAX, std::max(64, (max_read_length * 2 / 5 + 15) / 16 * 16)); }
+
 // Scratch capacities of tier t for reads of up to max_read_length bases: {minimizers, hits, candidates, draft mappings}.
 inline Caps tier_caps(int max_read_length, int t) {
   const int mrl = max_read_length;
-  const Caps c[N_TIERS] = {{mrl, 64, 32, 32}, {mrl * 2, 1024, 256, 256}, {mrl * 4, 65536, 8192, 8192}};
+  const Caps c[N_TIERS] = {{mrl, tier0_hits(mrl), 32, 32}, {mrl * 2, 1024, 256, 256}, {mrl * 4, 65536, 8192, 8192}};
   return c[t];
 }
 
@@ -205,8 +211,13 @@ void lane_emit(X &x, const LaneArgs &a, const LaneTiers &tiers, u32 batch_size) 
     const int g = (S.n_slots + TB - 1) / TB;
     x.emit_on(t);
     if (P.split) x(emit_split_kernel, g, TB, 0, P, a.R, a.B, a.T, S, a.sel, (OutPairs *)a.out_rec, a.out_n, a.ctr);
-    else if (a.sam && P.se) x(emit_sam_se_kernel, g, TB, 0, P, a.R, a.B, a.T, S, a.sel, (OutSam *)a.out_rec, a.out_n, a.ctr);
-    else if (a.sam) x(emit_sam_kernel, g, TB, 0, P, a.R, a.B, a.T, S, a.sel, (OutSam *)a.out_rec, a.out_n, a.ctr);
+    else if (a.sam) {
+      // the long instance's direction matrix is twice the local memory of the short one: only contexts sized for it use it
+      const bool sam_long = a.max_read_length > SAM_MAX_L;
+      const auto emit_sam = P.se ? (sam_long ? emit_sam_se_kernel<SAM_MAX_L_LONG> : emit_sam_se_kernel<SAM_MAX_L>)
+                                 : (sam_long ? emit_sam_kernel<SAM_MAX_L_LONG> : emit_sam_kernel<SAM_MAX_L>);
+      x(emit_sam, g, TB, 0, P, a.R, a.B, a.T, S, a.sel, (OutSam *)a.out_rec, a.out_n, a.ctr);
+    }
     else if (P.se) x(emit_se_kernel, g, TB, 0, P, a.R, a.B, a.T, S, a.sel, (OutRecord *)a.out_rec, a.out_n, a.ctr);
     else if (t > 0) x(emit_cta_kernel, S.n_slots, CTA_NT, 0, P, a.R, a.B, a.T, S, a.sel, (OutRecord *)a.out_rec, a.out_n, a.ctr);
     else {

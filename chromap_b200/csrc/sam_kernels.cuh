@@ -9,8 +9,9 @@
 #include "device_common.cuh"
 #endif
 
-#define SAM_MAX_L 160                 // reads up to 160 bases (2 x 150 bp fits); longer reads are reported, not aligned
-#define SAM_MAX_E 8                   // -e up to 8 (every preset that writes SAM); keeps the per-thread direction matrix at 35 x 160 bytes
+#define SAM_MAX_L 160                 // the short instance: reads up to 160 bases (2 x 150 bp fits)
+#define SAM_MAX_L_LONG 320            // the long instance, for contexts sized above 160 bases; longer reads are reported, not aligned
+#define SAM_MAX_E 8                   // -e up to 8 (every preset that writes SAM); keeps the per-thread direction matrix at 18 x MaxL bytes
 #define SAM_MAX_CIGAR 24              // == CMX_SAM_MAX_CIGAR
 
 #ifdef __CUDACC__
@@ -35,15 +36,16 @@
 // states, read back by the traceback exactly as ksw does.  WIN(j): base code of the window at j, RD(i): base code of the
 // read at i; scores: match / -mismatch between codes < 4, 0 if either is "other" (mapping_generator.h:661-670).
 // Returns the number of CIGAR operations (BAM encoding len << 4 | op, M = 0, I = 1, D = 2) or -1 if they do not fit `cap`.
+// MaxL: the longest read the direction matrix holds (rlen <= MaxL); it lives in local memory, 18 x MaxL bytes per thread.
 #define SAM_BAND (2 * SAM_MAX_E + 2)  // cells per row
-template <typename WinF, typename ReadF>
+template <int MaxL = SAM_MAX_L, typename WinF, typename ReadF>
 SAM_HD int sam_band_align(int rlen, int e, int match, int mismatch, int o_del, int e_del, int o_ins, int e_ins, WinF WIN, ReadF RD, unsigned int *cigar, int cap,
                           int *start, int *end) {
   const int NEG = -0x40000000;
   const int w = 2 * e + 1, wlen = rlen + 2 * e;
   const int oe_del = o_del + e_del, oe_ins = o_ins + e_ins;
   int hd[SAM_BAND], ed[SAM_BAND + 1];
-  unsigned char dirs[SAM_BAND * SAM_MAX_L];
+  unsigned char dirs[SAM_BAND * MaxL];
 #pragma unroll
   for (int d = 0; d < SAM_BAND; ++d) { hd[d] = 0; ed[d] = NEG; }  // free start on every diagonal of the band
   ed[SAM_BAND] = NEG;
@@ -102,12 +104,13 @@ struct OutSam {  // == cmx_sam_record
   u8 strand[2];        // 1 = +
   u8 mapq, is_unique, secondary;
   u8 n_cigar[2];
-  u8 overflow;         // read longer than SAM_MAX_L or CIGAR longer than SAM_MAX_CIGAR: reported, not written
+  u8 overflow;         // read longer than the instance's MaxL or CIGAR longer than SAM_MAX_CIGAR: reported, not written
   u32 cigar[2][SAM_MAX_CIGAR];
 };
 
 // SAM branch of GetRefStartEndPositionForReadFromMapping, non-split (mapping_generator.h:696-760 for the + strand,
 // :807-855 for the - strand: same call on the reverse complement with read_start_site = 0).  Returns false on overflow.
+template <int MaxL>
 __device__ __noinline__ bool sam_span(const DevParams &P, const DevRef &R, const u8 *read, int L, int strand, u64 dpos, u32 *st, u32 *en, u32 *cigar,
                                          u8 *n_cigar) {
   const int e = P.e;
@@ -115,14 +118,14 @@ __device__ __noinline__ bool sam_span(const DevParams &P, const DevRef &R, const
   u32 vws = rp + 1u > (u32)(L + e) ? rp + 1u - (u32)L - (u32)e : 0u;
   if (rp + (u32)e >= R.len[rid]) vws = R.len[rid] - (u32)e - (u32)L;
   *st = vws; *en = vws; *n_cigar = 0;
-  if (L > SAM_MAX_L || e > SAM_MAX_E) return false;
+  if (L > MaxL || e > SAM_MAX_E) return false;
   const u8 *win = R.seq + R.off[rid] + vws;
   int s0 = 0, e0 = 0, n;
   if (strand == 0)
-    n = sam_band_align(L, e, 1, 4, 6, 1, 6, 1, [&](int j) { return base_code(__ldg(win + j)); }, [&](int i) { return base_code(read[i]); }, cigar, SAM_MAX_CIGAR, &s0,
+    n = sam_band_align<MaxL>(L, e, 1, 4, 6, 1, 6, 1, [&](int j) { return base_code(__ldg(win + j)); }, [&](int i) { return base_code(read[i]); }, cigar, SAM_MAX_CIGAR, &s0,
                        &e0);
   else
-    n = sam_band_align(L, e, 1, 4, 6, 1, 6, 1, [&](int j) { return base_code(__ldg(win + j)); }, [&](int i) { return neg_code(read, L, i); }, cigar, SAM_MAX_CIGAR, &s0,
+    n = sam_band_align<MaxL>(L, e, 1, 4, 6, 1, 6, 1, [&](int j) { return base_code(__ldg(win + j)); }, [&](int i) { return neg_code(read, L, i); }, cigar, SAM_MAX_CIGAR, &s0,
                        &e0);
   *st = vws + (u32)s0;
   *en = vws + (u32)e0 - 1u;
@@ -133,6 +136,7 @@ __device__ __noinline__ bool sam_span(const DevParams &P, const DevRef &R, const
 
 // emit_kernel with the SAM span: ProcessBestMappingsForPairedEndReadOnOneDirection (mapping_generator.h:486-654) + the fields
 // EmplaceBackPairedEndMappingRecord<SAMMapping> needs (mapping_generator.cc:84-107); flags and TLEN are derived on the host.
+template <int MaxL>
 __global__ void emit_sam_kernel(DevParams P, DevRef R, DevBatch B, MapqTables T, Scratch S, const int *pair_sel, OutSam *out, int *out_n, Counters *ctr) {
   const int slot = blockIdx.x * blockDim.x + threadIdx.x;
   if (slot >= S.n_slots) return;
@@ -158,8 +162,8 @@ __global__ void emit_sam_kernel(DevParams P, DevRef R, DevBatch B, MapqTables T,
       if (idx == sel[reported]) {
         OutSam &o = out[(size_t)pair * mb + reported];
         u32 st1, en1, st2, en2;
-        const bool ok1 = sam_span(P, R, rd[0], L[0], s1, p1[i1], &st1, &en1, o.cigar[0], &o.n_cigar[0]);
-        const bool ok2 = sam_span(P, R, rd[1], L[1], s2, p2[j], &st2, &en2, o.cigar[1], &o.n_cigar[1]);
+        const bool ok1 = sam_span<MaxL>(P, R, rd[0], L[0], s1, p1[i1], &st1, &en1, o.cigar[0], &o.n_cigar[0]);
+        const bool ok2 = sam_span<MaxL>(P, R, rd[1], L[1], s2, p2[j], &st2, &en2, o.cigar[1], &o.n_cigar[1]);
         const unsigned short al1 = (unsigned short)(en1 - st1 + 1u), al2 = (unsigned short)(en2 - st2 + 1u);
         o.read_id = B.first_read_id + (u32)pair;
         o.rid = (u32)(p1[i1] >> 32);
@@ -182,6 +186,7 @@ __global__ void emit_sam_kernel(DevParams P, DevRef R, DevBatch B, MapqTables T,
 }
 
 // emit_se_kernel with the SAM span (mapping_generator.h:256-343 with MAPPINGFORMAT_SAM)
+template <int MaxL>
 __global__ void emit_sam_se_kernel(DevParams P, DevRef R, DevBatch B, MapqTables T, Scratch S, const int *pair_sel, OutSam *out, int *out_n, Counters *ctr) {
   const int slot = blockIdx.x * blockDim.x + threadIdx.x;
   if (slot >= S.n_slots) return;
@@ -203,7 +208,7 @@ __global__ void emit_sam_se_kernel(DevParams P, DevRef R, DevBatch B, MapqTables
       if (idx == sel[reported]) {
         OutSam &o = out[(size_t)pair * mb + reported];
         u32 st, en;
-        const bool ok = sam_span(P, R, r, L, s, mp[mi], &st, &en, o.cigar[0], &o.n_cigar[0]);
+        const bool ok = sam_span<MaxL>(P, R, r, L, s, mp[mi], &st, &en, o.cigar[0], &o.n_cigar[0]);
         const unsigned short al = (unsigned short)(en - st + 1u);
         o.read_id = B.first_read_id + (u32)pair;
         o.rid = (u32)(mp[mi] >> 32);

@@ -50,7 +50,8 @@ typedef struct {
   int32_t output_format;          /* 1 = BED, 2 = TagAlign (same records), 4 = SAM cores (cmx_sam_record), 5 = pairs (mapping_parameters.h:9-16) */
   int32_t batch_size;             /* pairs per reference batch (chromap.h:182: 500000); fixes the
                                      taskloop chunking that seeds multi-mapper sampling */
-  int32_t max_read_length;        /* upper bound on read length in any batch (sizing), default 160 */
+  int32_t max_read_length;        /* scratch sizing, default 160, at most 843 on an H100 (320 with SAM output); reads up to 2x / 4x as
+                                     long go to overflow tiers sized for a few of them (cmx_set_max_read_length resizes a live context) */
   int32_t single_end;             /* 1 = single-end reads (chromap -1 only; MapSingleEndReads, chromap.h:218-634): cmx_batch.seq2/off2
                                      are NULL, records are MappingWithoutBarcode (both alignment lengths 0). BED, non-split only */
 } cmx_params;
@@ -430,6 +431,13 @@ int cmx_host_unregister(void *ptr);
  * cmx_timing's stage times are exclusive; with more lanes they are sums over overlapping streams.  Changing the
  * count releases the lanes' scratch tiers (they grow again at the next call), so device memory follows the new split. */
 int cmx_set_lanes(cmx_ctx *ctx, int n_lanes);
+
+/* Resize a live context for reads of up to L bases, as if it had been created with max_read_length = L: every later call
+ * gives exactly the records of a context created with L.  Waits for the device, then releases the lanes' scratch tiers
+ * (they grow again at the next call).  CMX_ERR_INVALID, with the context unchanged, for L < min_read_length, L > 1600,
+ * L > 320 with SAM output (output_format 4), or an L whose front-end read tiles (64 reads) do not fit the device's shared
+ * memory: above 843 bases on an H100.  A context never resized keeps the size it was created with. */
+int cmx_set_max_read_length(cmx_ctx *ctx, int32_t L);
 
 
 /* ---- multi-GPU: the one exchange step (SURVEY.md 8e) ---------------------------------------------------------------------
