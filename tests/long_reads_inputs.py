@@ -5,7 +5,7 @@ Fragments are drawn uniformly from the reference, both strands, with about 1 % s
 Kinds:
   pe<L>   pairs of L-base mates, fragments of max(L - 60, L / 2) .. 3L bases: the shortest read into the Nextera adapter, which
           `--preset atac` trims;
-  mixed   pairs whose mates are 50 .. 300 bases each, independently;
+  mixed   pairs whose mates are 50 .. 300 bases each, independently; mixed<M>: 50 .. M bases;
   se<L>   read 1 of pe<L>;
   hic<L>  Hi-C-like pairs: mates from two loci, a third of read 1 chimeric (its tail from read 2's locus).
 Barcodes (`barcodes`) are drawn from synth_sc's whitelist, one in ten with one substitution."""
@@ -61,8 +61,9 @@ def make_pairs(kind, n, seed, seqs=None):
         _, seqs = read_fasta(REF)
     out = []
     for _ in range(n):
-        if kind == "mixed":
-            l1, l2 = int(g.integers(50, 301)), int(g.integers(50, 301))
+        if kind.startswith("mixed"):
+            hi = int(kind[5:] or 300)
+            l1, l2 = int(g.integers(50, hi + 1)), int(g.integers(50, hi + 1))
             f = _frag(g, seqs, int(g.integers(max(l1, l2), 3 * max(l1, l2) + 1)))
             out.append((_mutate(g, f[:l1]), _mutate(g, f.translate(COMP)[::-1][:l2])))
         elif kind.startswith("hic"):
@@ -113,6 +114,8 @@ def write_set(d, kind, n, seed, tag=None):
 
 # the golden inputs: kind -> (pairs, seed)
 GOLDEN_SETS = {"pe250": (5000, 250), "pe300": (4000, 300), "mixed": (5000, 77), "se250": (5000, 251), "hic250": (4000, 252)}
+# reads beyond 320 bases, written where a test runs (the reference binary maps them there): kind -> (pairs, seed)
+BEYOND_320_SETS = {"pe400": (2000, 400), "pe600": (1500, 600), "pe832": (1000, 832), "mixed1400": (1500, 1400), "se600": (1500, 601), "hic400": (1500, 402)}
 
 
 if __name__ == "__main__":

@@ -31,9 +31,12 @@ static std::string mutate(const std::string &ref, int off, int L, int n_edit, bo
 }
 int main() {
   srand(23);
-  long bad = 0, n_align = 0, n_tb = 0, n_drop = 0, n_dp = 0;
+  long bad = 0, n_align = 0, n_tb = 0, n_drop = 0, n_dp = 0, n_long = 0, n_long_tb = 0, n_long_drop = 0;
   for (int it = 0; it < 200000; ++it) {
-    const int e = 1 + rand() % 15, L = 25 + rand() % 140;
+    // one window in eight from a read beyond 164 bases: up to 4 x 832 (the last overflow tier's reads) and a little over
+    const bool long_read = rand() % 8 == 0;
+    const int e = 1 + rand() % 15, L = long_read ? 165 + rand() % 3236 : 25 + rand() % 140;
+    n_long += long_read;
     std::string ref(L + 2 * e + 64, 'A');
     for (auto &c : ref) c = "ACGT"[rand() % 4];
     if (rand() % 8 == 0) for (auto &c : ref) c = "AC"[rand() % 2];
@@ -55,6 +58,7 @@ int main() {
         orc_banded_traceback(e, r1, ref.data() + vws, read.data(), L, &s1);
         const int s2 = banded_traceback(e, r1, L, [&](int i) { return (u8)ref[vws + i]; }, [&](int i) { return (u8)read[i]; });
         ++n_tb;
+        n_long_tb += long_read;
         int ham = 0;
         for (int i = 0; i < L; ++i) ham += ref[vws + e + i] != read[i];
         if (r1 != 0 && ham != r1) ++n_dp;
@@ -71,11 +75,13 @@ int main() {
         const int d1 = orc_align_dropoff(e, ref.data(), txt.data(), L, from3, &a1, &b1);
         const int d2 = banded_align_dropoff(e, L, from3 != 0, [&](int i) { return base_code((u8)ref[i]); }, [&](int i) { return base_code((u8)txt[i]); }, &a2, &b2);
         ++n_drop;
+        n_long_drop += long_read;
         if (d1 != d2 || a1 != a2 || b1 != b2) { if (bad < 5) printf("DROPOFF e=%d L=%d from3=%d err %d/%d end %d/%d len %d/%d\n", e, L, from3, d1, d2, a1, a2, b1, b2); ++bad; }
       }
     }
   }
-  printf("aligned=%ld tracebacks=%ld (bit-vector path %ld) dropoffs=%ld bad=%ld\n", n_align, n_tb, n_dp, n_drop, bad);
+  printf("aligned=%ld tracebacks=%ld (bit-vector path %ld) dropoffs=%ld long=%ld long_tracebacks=%ld long_dropoffs=%ld bad=%ld\n", n_align, n_tb, n_dp, n_drop, n_long,
+         n_long_tb, n_long_drop, bad);
   return bad != 0;
 }
 '''
@@ -87,3 +93,4 @@ def test_device_banded_aligners_equal_the_oracle(tmp_path):
     # the interesting branches were really taken
     f = dict(kv.split("=") for kv in out.stdout.replace("(bit-vector path ", "dp=").replace(")", "").split() if "=" in kv)
     assert int(f["dp"]) > 1000 and int(f["tracebacks"]) - int(f["dp"]) > 10000 and int(f["dropoffs"]) > 10000, out.stdout
+    assert int(f["long"]) > 20000 and int(f["long_tracebacks"]) > 5000 and int(f["long_dropoffs"]) > 5000, out.stdout

@@ -2,9 +2,11 @@
 
 Library: the same batches through a context created at the default 160 bases and grown by cmx_set_max_read_length, a
 context created at the final length, and the oracle: identical records for BED, SAM cores, Hi-C pairs and single-end.
-Refused sizes leave the context as it was.  CLI: every golden with the device and the host reader; a run of two file sets,
-2x50 then 2x250 (`-1 a,b`), so that the context grows between them, against the reference binary run at test time; and a
-`--SAM` run that meets a 400-base read stops without writing its output file."""
+Beyond 320 bases (seeded reads, tests/long_reads_inputs.py): contexts of 416, 608 and 832 bases, one created at 843 (the
+device bound), and mates of up to 1,400 bases at 832 through the overflow tiers.  Refused sizes leave the context as it was.
+CLI: every golden with the device and the host reader; a run of two file sets, 2x50 then 2x250 (`-1 a,b`), so that the
+context grows between them, and runs of 2x400, 2x832 and mates of 50 to 1,400 bases, each against the reference binary run
+at test time; and a `--SAM` run that meets a 400-base read stops without writing its output file."""
 import gzip
 import os
 import subprocess
@@ -14,7 +16,7 @@ import pytest
 
 import chromap_b200 as cb
 from oracle import oracle_py as orc
-from tests.long_reads_inputs import make_pairs, write_fastq, write_set
+from tests.long_reads_inputs import BEYOND_320_SETS, make_pairs, write_fastq, write_set
 from tests.test_gpu_parity import assert_same_records
 from tests.test_oracle_long import CASES
 from tests.util import load_pairs, pack, read_fasta
@@ -65,7 +67,27 @@ LIB_CASES = {
     "pe250_sam": ("pe250", 256, "sam", "", dict(mapq_threshold=0)),
     "se250_sam": ("se250", 256, "sam", "", dict(mapq_threshold=0)),
     "hic250": ("hic250", 256, "pairs", "hic", {}),
+    "pe400_chip": ("pe400", 416, "bed", "chip", {}),
+    "pe600_chip": ("pe600", 608, "bed", "chip", {}),
+    "pe600_atac": ("pe600", 608, "bed", "atac", {}),
+    "pe832_chip": ("pe832", 832, "bed", "chip", {}),
+    "se600_chip": ("se600", 608, "bed", "chip", {}),
+    "hic400": ("hic400", 416, "pairs", "hic", {}),
 }
+
+
+def _reads(data, reads):
+    """(s1, o1, s2, o2) of a golden read set, or of a set beyond 320 bases drawn from its seed (s2 = o2 = None: single-end)."""
+    if reads not in BEYOND_320_SETS:
+        se = reads.startswith("se")
+        s1, o1, s2, o2 = load_pairs(data["d"], reads + "_1.fq.gz", reads + "_1.fq.gz" if se else reads + "_2.fq.gz")
+        return (s1, o1, None, None) if se else (s1, o1, s2, o2)
+    pairs = make_pairs(reads, *BEYOND_320_SETS[reads])
+    s1, o1 = pack([a for a, _ in pairs])
+    if pairs[0][1] is None:
+        return s1, o1, None, None
+    s2, o2 = pack([b for _, b in pairs])
+    return s1, o1, s2, o2
 
 
 @pytest.mark.parametrize("case", sorted(LIB_CASES))
@@ -73,21 +95,20 @@ def test_grown_context_equals_created_context_and_oracle(long_data, case):
     reads, L, out, preset, kw = LIB_CASES[case]
     se = reads.startswith("se")
     kw = dict(kw, single_end=int(se), output_format=4 if out == "sam" else cb.make_params(preset).output_format)
-    s1, o1, s2, o2 = load_pairs(long_data["d"], reads + "_1.fq.gz", reads + "_1.fq.gz" if se else reads + "_2.fq.gz")
-    if se:
-        s2 = o2 = None
+    s1, o1, s2, o2 = _reads(long_data, reads)
     op = orc.make_params(preset, **{k: v for k, v in kw.items() if k != "output_format" or v != 4})  # the oracle's SAM cores take BED params
     grown = _mapper(long_data, preset, 160, **kw)
+    before = None
     if out == "sam":  # at 160 bases the SAM cores of longer reads are reported as overflowed, not aligned
         with pytest.raises(cb.CmxError):
             grown.map_batch(s1, o1, s2, o2, first_read_id=7)
-    else:  # every pair through the overflow tiers: the same records, only more slowly
+    elif L <= 4 * 160:  # every pair through the overflow tiers: the same records, only more slowly (the last tier takes 640 bases)
         before, _ = grown.map_batch(s1, o1, s2, o2, first_read_id=7)
     grown.set_max_read_length(L)
     created = _mapper(long_data, preset, L, **kw)
     got = [m.map_batch(s1, o1, s2, o2, first_read_id=7) for m in (grown, created)]
     for recs, stats in got:
-        assert stats["n_overflow_pairs"] == 0 and len(recs) > 2000
+        assert stats["n_overflow_pairs"] == 0 and len(recs) > (2000 if reads not in BEYOND_320_SETS else (len(o1) - 1) // 4)
     if out == "sam":
         cores = orc.map_sam_cores(op, long_data["oidx"], long_data["oref"], s1, o1, s2, o2, first_read_id=7)
         for recs, _ in got:
@@ -99,7 +120,36 @@ def test_grown_context_equals_created_context_and_oracle(long_data, case):
             want, _ = orc.map_pairs(op, long_data["oidx"], long_data["oref"], s1, o1, s2, o2, first_read_id=7)
         for recs, _ in got:
             assert_same_records(recs, want)
-        assert_same_records(before, want)
+        if before is not None:
+            assert_same_records(before, want)
+
+
+def test_context_created_at_the_device_bound(long_data):
+    """843 bases, the longest a context can be sized for (the front end's tiles then take 232,320 B of the 232,448 B of
+    shared memory an H100 grants a CTA): 2x832 pairs stay out of the overflow tiers' refusal and map as the oracle does."""
+    s1, o1, s2, o2 = _reads(long_data, "pe832")
+    m = _mapper(long_data, "chip", 843)
+    recs, stats = m.map_batch(s1, o1, s2, o2)
+    print("tier pairs at 843:", m.timing()["tier_pairs"])
+    assert stats["n_overflow_pairs"] == 0 and len(recs) > (len(o1) - 1) // 4
+    want, _ = orc.map_pairs(orc.make_params("chip"), long_data["oidx"], long_data["oref"], s1, o1, s2, o2)
+    assert_same_records(recs, want)
+
+
+def test_mates_beyond_the_context_take_the_overflow_tiers(long_data):
+    """Mates of 50 to 1,400 bases at 832: every pair with a mate over 832 bases goes to tier 1 (maxmm 1,664), and repeats of
+    synth_sc's reference push some pairs on to tier 2 (maxmm 3,328), where the CTA kernels meet their largest shared-memory
+    requests; the records are the oracle's."""
+    s1, o1, s2, o2 = _reads(long_data, "mixed1400")
+    n_long = int(np.sum((np.diff(o1) > 832) | (np.diff(o2) > 832)))
+    m = _mapper(long_data, "chip", 832)
+    recs, stats = m.map_batch(s1, o1, s2, o2)
+    t = m.timing()["tier_pairs"]
+    print("tier pairs at 832, mates of up to 1,400 bases:", t, "pairs with a mate over 832:", n_long)
+    assert n_long > 100 and t[1] >= n_long and t[2] > 0 and stats["n_overflow_pairs"] == 0, t
+    want, _ = orc.map_pairs(orc.make_params("chip"), long_data["oidx"], long_data["oref"], s1, o1, s2, o2)
+    assert len(want) > 300
+    assert_same_records(recs, want)
 
 
 def test_grown_context_keeps_long_pairs_in_tier_0():
@@ -205,6 +255,25 @@ def test_cli_grows_between_file_sets_like_the_reference(cli_data, reader):
     assert p.stderr.count("mapping scratch resized for 256-base reads") == 1
     w = open(want, "rb").read()
     assert w.count(b"\n") > 3000 and open(got, "rb").read() == w
+
+
+@pytest.mark.parametrize("reader", ["device", "host"])
+@pytest.mark.parametrize("kind,resized", [("pe400", 416), ("pe832", 832), ("mixed1400", 832)])
+def test_cli_equals_reference_beyond_320_bases(cli_data, kind, resized, reader):
+    """2x400, 2x832 and mates of 50 to 1,400 bases (the context stops at 832; longer mates take the overflow tiers)."""
+    if not os.path.exists(REF_BIN):
+        pytest.skip("oracle/_ref/chromap not built")
+    t = cli_data["t"]
+    r1, r2 = write_set(str(t), kind, *BEYOND_320_SETS[kind])
+    args = ["--preset", "chip", "-x", cli_data["idx"], "-r", cli_data["ref"], "-1", r1, "-2", r2]
+    want, got = str(t / ("ref_%s.bed" % kind)), str(t / ("%s_%s.bed" % (reader, kind)))
+    if not os.path.exists(want):
+        subprocess.check_call([REF_BIN, "-t", "1", "-o", want] + args, stderr=subprocess.DEVNULL)
+    p = subprocess.run([CLI, "-o", got] + args + (["--host-reader"] if reader == "host" else []), capture_output=True, text=True)
+    assert p.returncode == 0, p.stderr[-2000:]
+    assert p.stderr.count("mapping scratch resized for %d-base reads" % resized) == 1, p.stderr[-2000:]
+    w = open(want, "rb").read()
+    assert w.count(b"\n") > 300 and open(got, "rb").read() == w
 
 
 def test_cli_sam_refuses_reads_longer_than_320_before_writing(cli_data):

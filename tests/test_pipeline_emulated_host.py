@@ -60,8 +60,12 @@ struct EmuLane {
   std::vector<char> lists[LIST_OVERFLOW + N_TIERS];
   int cnt[4] = {0, 0, 0, 0};
   std::vector<int> chunks;
+  size_t max_smem = 0;   // the largest dynamic shared memory a launch asked for
+  int cluster_launches = 0;
   template <typename... KA, typename... A>
   void operator()(void (*kernel)(KA...), int grid, int block, size_t smem, A... a) {
+    max_smem = std::max(max_smem, smem);
+    if ((void *)kernel == (void *)&cluster_kernel) ++cluster_launches;
     g_smem = std::vector<u64>((smem + 7) / 8, 0xA5A5A5A5A5A5A5A5ull);
     g_dyn_smem = g_smem.data();
     emu_grid(grid, block, [&]() { kernel(a...); });
@@ -87,13 +91,20 @@ struct RunStats {
   // below the start of a rid > 0 (`lookup_at_start`: a mate without candidates of its own mapped by the lookup, the whole fragment
   // within 2 * max_insert of the rid's start, so the partner's candidate lies there too)
   long edge_start = 0, edge_end = 0, short_seq = 0, lookup_at_start = 0;
+  // front-end tiles (per mate) too long to stage, read by each thread from global memory (seed_front_kernel's own test
+  // g1 - base > tb); reads that cluster_kernel's first pass listed for the second; reads of mapped pairs with 256 or more
+  // minimizers (the oracle's count: candidate counts are u8 and wrap there); the launches' largest dynamic shared memory
+  long unstaged = 0, second_pass = 0, mm256 = 0, max_smem = 0, cluster_launches = 0;
 };
 
 enum { MODE_CHIP = 0, MODE_ATAC = 1, MODE_HIC = 2, MODE_SE = 3, MODE_SAM = 4, MODE_SAM_SE = 5 };
 // mapping knobs over the preset (-1: the preset's value): -e, -s, -f f0,f1, --drop-repetitive-reads, --min-read-length
 struct Knobs { int e = -1, min_seeds = -1, f0 = -1, f1 = -1, drop_rep = -1, min_read_len = -1; };
 static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *caps3, int max_best, int read_len_base, bool front_only = false, int K = 17, int W = 7, int fam_copies = 90,
-                         const Knobs &kn = Knobs{}, bool edges = false) {
+                         const Knobs &kn = Knobs{}, bool edges = false, bool exact_len = false, int over_lo = 0, int over_hi = 0) {
+  // exact_len: every read read_len_base bases (no spread); over-long reads (one pair in twenty) of over_lo .. over_hi bases
+  // (0: mrl + 5 .. mrl + 44)
+  if (over_lo == 0) { over_lo = mrl + 5; over_hi = mrl + 44; }
   std::mt19937 g((unsigned)seed);
   RunStats rs;
   // ---- reference: two sequences, a 300 bp family with many copies, a 2 kb segmental repeat, an N run
@@ -131,7 +142,8 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   for (int p = 0; p < n_pairs; ++p) {
     const int kind = (int)(g() %% 20);
     int L1 = read_len_base + (int)(g() %% 11) - 5, L2 = read_len_base + (int)(g() %% 11) - 5;
-    if (kind == 0) L1 = mrl + 5 + (int)(g() %% 40);                   // longer than the first tier allows
+    if (exact_len) L1 = L2 = read_len_base;
+    if (kind == 0) L1 = over_lo + (int)(g() %% (unsigned)(over_hi - over_lo + 1));   // longer than the first tier allows
     if (kind == 1) L2 = 20;                                           // below the length filter
     const std::string &rsq = seq[g() %% (edges ? n_seq : 2)];
     int frag = std::max(L1, L2) + (int)(g() %% 350);
@@ -268,6 +280,29 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   for (int t = 0; t < N_TIERS; ++t) x.tiers[t].caps = caps3[t];
   const LaneArgs a{P, ix, R, B, T, mt_init, &ctr, x.cnt, nbest.data(), sel.data(), out_n.data(), is_sam ? (void *)out_sam.data() : (void *)out_rec.data(), is_sam, mrl};
   g_emu_leavable = true;
+  {   // the tiles seed_front_kernel cannot stage (one grid over all pairs: tiles start at slot 0)
+    const size_t tb = seed_front_tile_bytes(caps3[0].maxmm);
+    for (int p0 = 0; p0 < n; p0 += SF_TILE)
+      for (int m = 0; m < (is_se ? 1 : 2); ++m) {
+        const std::string &sq = m == 0 ? s1 : s2;
+        const std::vector<u32> &of = m == 0 ? o1 : o2;
+        const u64 g0 = (u64)(sq.data() + of[(size_t)p0]), g1 = (u64)(sq.data() + of[(size_t)std::min(n, p0 + SF_TILE)]);
+        rs.unstaged += g1 - (g0 & ~15ull) > tb;
+      }
+  }
+  for (int p = 0; p < n; ++p) {   // mapped reads with 256 or more minimizers
+    bool mapped = false;
+    if (is_sam) { for (long i = 0; i < n_want_sam; ++i) mapped |= want_sam[i].read_id == first_read_id + (u32)p; }
+    else if (mode == MODE_HIC) { for (long i = 0; i < n_want; ++i) mapped |= ((const orc_pairs_record *)want.data())[i].read_id == first_read_id + (u32)p; }
+    else for (long i = 0; i < n_want; ++i) mapped |= want[i].read_id == first_read_id + (u32)p;
+    if (!mapped) continue;
+    for (int m = 0; m < (is_se ? 1 : 2); ++m) {
+      std::vector<uint64_t> mh(8192), mhit(8192);
+      const char *rd = m == 0 ? s1.data() + o1[p] : s2.data() + o2[p];
+      const u32 len = m == 0 ? o1[p + 1] - o1[p] : o2[p + 1] - o2[p];
+      rs.mm256 += orc_minimizers(rd, len, 0, K, W, mh.data(), mhit.data(), 8192) >= 256;
+    }
+  }
   // the front end: [adapter trimming] + length filter + minimizers + table probes over staged read tiles (seed_front_kernel, a
   // persistent grid: three CTAs here, so that every CTA walks several tiles through both stages of its double buffer)
   const Scratch S = lane_front(x, a, (u32)n, front_only ? 2 : 3);
@@ -301,9 +336,11 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   }
   const LaneTiers tiers = lane_tiers(x, a, S);
   for (int t = 0; t < tiers.used; ++t) rs.tier_pairs[t] = tiers.S[t].n_slots;
+  rs.second_pass = x.cnt[3];   // (cluster_kernel's list counter: nothing after tier 0's clustering clears it)
   if (tiers.n_left > 0) { printf("pairs left after the last tier: %%d\n", tiers.n_left); ++rs.bad; }
   lane_emit(x, a, tiers, (u32)n);   // all pairs one reference batch
   g_emu_leavable = false;
+  rs.max_smem = (long)x.max_smem; rs.cluster_launches = x.cluster_launches;
   // ---- compare, pair by pair
   if (is_sam) {
     static_assert(sizeof(OutSam) == sizeof(orc_sam_record), "SAM record layout");
@@ -354,14 +391,17 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
 
 int main(int argc, char **argv) {
   static_assert(sizeof(OutRecord) == sizeof(orc_pe_record) && sizeof(OutPairs) == sizeof(orc_pe_record), "record layouts");
-  const bool want_edges = argc > 1 && !strcmp(argv[1], "edges");   // the runs at the ends of reference sequences, else all others
+  // the runs at the ends of reference sequences ("edges"), at the sizes a context grown beyond 160 bases takes ("grown"), else all others
+  const bool want_edges = argc > 1 && !strcmp(argv[1], "edges"), want_grown = argc > 1 && !strcmp(argv[1], "grown");
   long bad = 0;
   const int mrl = 80;
   const Caps real[3] = {tier_caps(mrl, 0), tier_caps(mrl, 1), tier_caps(mrl, 2)};   // the library's tiers
   const Caps small[3] = {{mrl, 6, 2, 2}, {mrl * 2, 40, 6, 6}, {mrl * 4, 65536, 8192, 8192}};            // most pairs through the CTA kernels, some to the last tier
   const Caps real_long[3] = {tier_caps(150, 0), tier_caps(150, 1), tier_caps(150, 2)};
   const Caps small_long[3] = {{150, 6, 2, 2}, {300, 40, 6, 6}, {600, 65536, 8192, 8192}};
-  struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; Knobs knobs = {}; bool edges = false; };
+  const Caps small_256[3] = {{256, 6, 2, 2}, {512, 40, 6, 6}, {1024, 65536, 8192, 8192}};
+  struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; Knobs knobs = {}; bool edges = false;
+                bool grown = false, exact = false; int over_lo = 0, over_hi = 0; };   // grown: caps nullptr = the library's tiers at mrl
   const Case cases[] = {
       {"real_tiers", MODE_CHIP, 3, 100, 1, 60, real, mrl},
       {"small_first_tier", MODE_CHIP, 4, 48, 3, 60, small, mrl},
@@ -414,14 +454,43 @@ int main(int argc, char **argv) {
       {"edges_sam", MODE_SAM, 48, 160, 2, 60, real, mrl, false, 17, 7, 90, {}, true},
       {"edges_sam_single_end", MODE_SAM_SE, 49, 160, 2, 60, real, mrl, false, 17, 7, 90, {}, true},
       {"edges_f3_40", MODE_CHIP, 50, 300, 2, 60, real, mrl, false, 17, 7, 90, Knobs{.f0 = 3, .f1 = 40}, true},
+      // contexts of 192 to 832 bases with the library's tiers: tier 0's hit rows 80 (192), 112 (256), 192 (from 448); two
+      // cluster launches while the first-pass tile is shorter than hc (448, 704), one from 736; whole read-length tiles,
+      // so that a tile with an over-long read is not staged (448 and up); at 832 the front end's tiles take 229,504 B and one
+      // pair in twenty has a mate of 1,050 to 1,400 bases: the overflow tiers at maxmm 1,664 / 3,328, 256 or more minimizers
+      {.name = "grown_chip192", .mode = MODE_CHIP, .seed = 60, .n = 96, .max_best = 1, .len = 186, .caps = nullptr, .mrl = 192, .fam_copies = 30, .grown = true},
+      {.name = "grown_chip256", .mode = MODE_CHIP, .seed = 61, .n = 96, .max_best = 2, .len = 250, .caps = nullptr, .mrl = 256, .fam_copies = 30, .grown = true},
+      {.name = "grown_chip448", .mode = MODE_CHIP, .seed = 62, .n = 80, .max_best = 1, .len = 448, .caps = nullptr, .mrl = 448, .fam_copies = 20, .grown = true, .exact = true},
+      {.name = "grown_chip704", .mode = MODE_CHIP, .seed = 63, .n = 128, .max_best = 1, .len = 704, .caps = nullptr, .mrl = 704, .fam_copies = 10, .grown = true, .exact = true},
+      {.name = "grown_chip736", .mode = MODE_CHIP, .seed = 64, .n = 80, .max_best = 1, .len = 736, .caps = nullptr, .mrl = 736, .fam_copies = 10, .grown = true, .exact = true},
+      {.name = "grown_chip832", .mode = MODE_CHIP, .seed = 65, .n = 160, .max_best = 2, .len = 832, .caps = nullptr, .mrl = 832, .fam_copies = 20, .grown = true, .exact = true,
+       .over_lo = 1050, .over_hi = 1400},
+      // adapter trimming before the front end (prepped = 1), single-end, Hi-C split alignment in the thread and the CTA form
+      {.name = "grown_atac256", .mode = MODE_ATAC, .seed = 66, .n = 80, .max_best = 1, .len = 250, .caps = nullptr, .mrl = 256, .fam_copies = 30, .grown = true},
+      {.name = "grown_single_end320", .mode = MODE_SE, .seed = 67, .n = 96, .max_best = 2, .len = 314, .caps = nullptr, .mrl = 320, .fam_copies = 30, .grown = true},
+      {.name = "grown_hic256", .mode = MODE_HIC, .seed = 68, .n = 64, .max_best = 1, .len = 250, .caps = nullptr, .mrl = 256, .fam_copies = 30, .grown = true},
+      {.name = "grown_hic256_cta", .mode = MODE_HIC, .seed = 69, .n = 24, .max_best = 1, .len = 250, .caps = small_256, .mrl = 256, .fam_copies = 30, .grown = true},
+      // --SAM above 160 bases: emit_sam_kernel<320> / emit_sam_se_kernel<320>, as lane_emit picks them (SAM reads stay within 320)
+      {.name = "grown_sam256", .mode = MODE_SAM, .seed = 70, .n = 64, .max_best = 2, .len = 250, .caps = nullptr, .mrl = 256, .fam_copies = 30, .grown = true},
+      {.name = "grown_sam_single_end320", .mode = MODE_SAM_SE, .seed = 71, .n = 64, .max_best = 2, .len = 300, .caps = nullptr, .mrl = 320, .fam_copies = 30, .grown = true,
+       .over_lo = 306, .over_hi = 320},
+      // k = 23: no key rows in the front end, the run-time scan, the first-pass tile by w = 11; then tiny first tiers: most
+      // pairs through the CTA kernels at maxmm 512 / 1,024
+      {.name = "grown_k23_w11_320", .mode = MODE_CHIP, .seed = 72, .n = 96, .max_best = 1, .len = 314, .caps = nullptr, .mrl = 320, .k = 23, .w = 11, .fam_copies = 30, .grown = true},
+      {.name = "grown_small_tiers256", .mode = MODE_CHIP, .seed = 73, .n = 48, .max_best = 3, .len = 250, .caps = small_256, .mrl = 256, .fam_copies = 30, .grown = true},
   };
   const int seed_off = getenv("EMU_SEED_OFFSET") ? atoi(getenv("EMU_SEED_OFFSET")) : 0;   // other inputs of the same kinds (offline fuzzing)
   for (const Case &c : cases) {
-    if (c.edges != want_edges) continue;
-    const RunStats r = run_case(c.mode, c.seed + seed_off, c.n, c.mrl, c.caps, c.max_best, c.len, c.front_only, c.k, c.w, c.fam_copies, c.knobs, c.edges);
-    printf("%%s: pairs=%%ld records=%%ld tier0=%%ld tier1=%%ld tier2=%%ld bad=%%ld edge_start=%%ld edge_end=%%ld short_seq=%%ld lookup_at_start=%%ld\n", c.name, r.pairs, r.records,
-           r.tier_pairs[0], r.tier_pairs[1], r.tier_pairs[2], r.bad, r.edge_start, r.edge_end, r.short_seq, r.lookup_at_start);
+    if (c.edges != want_edges || c.grown != want_grown) continue;
+    Caps lib[3];
+    for (int t = 0; t < 3; ++t) lib[t] = tier_caps(c.mrl, t);
+    const RunStats r = run_case(c.mode, c.seed + seed_off, c.n, c.mrl, c.caps ? c.caps : lib, c.max_best, c.len, c.front_only, c.k, c.w, c.fam_copies, c.knobs, c.edges, c.exact,
+                                c.over_lo, c.over_hi);
+    printf("%%s: pairs=%%ld records=%%ld tier0=%%ld tier1=%%ld tier2=%%ld bad=%%ld edge_start=%%ld edge_end=%%ld short_seq=%%ld lookup_at_start=%%ld unstaged=%%ld second_pass=%%ld "
+           "mm256=%%ld max_smem=%%ld cluster_launches=%%ld\n", c.name, r.pairs, r.records, r.tier_pairs[0], r.tier_pairs[1], r.tier_pairs[2], r.bad, r.edge_start, r.edge_end,
+           r.short_seq, r.lookup_at_start, r.unstaged, r.second_pass, r.mm256, r.max_smem, r.cluster_launches);
     bad += r.bad;
+    if (r.max_smem > 232448) { printf("%%s: a launch asks for %%ld B of dynamic shared memory, more than an H100 grants a CTA (232,448 B)\n", c.name, r.max_smem); ++bad; }
   }
   printf("total_bad=%%ld\n", bad);
   return bad != 0;
@@ -488,3 +557,30 @@ def test_device_pipeline_at_sequence_ends_equals_the_oracle(tmp_path):
     # and over all runs
     total = [sum(got[name][i] for name in floors) for i in (4, 5, 6)]
     assert total[0] >= 15 and total[1] >= 35 and total[2] >= 22, (total, out.stdout)
+
+
+def test_device_pipeline_at_grown_read_lengths_equals_the_oracle(tmp_path):
+    """Contexts of 192 to 832 bases, with the tiers the library sizes for them (`tier_caps`): tier 0's hit rows of 80, 112
+    and 192, one or two cluster_kernel passes, front-end tiles too long to stage (each thread then copies its own read), the
+    overflow tiers at maxmm up to 3,328 with reads of 256 or more minimizers, adapter trimming, single-end, Hi-C in the thread
+    and the CTA form, `--SAM` through the 320-base instances, k = 23 and tiny first tiers.  Each run must show that it reached
+    what it is there for, and no launch may ask for more dynamic shared memory than an H100 grants one CTA (232,448 B)."""
+    out = _run_cases(tmp_path, ["grown"])
+    got = {m.group(1): [int(x) for x in m.groups()[1:]] for m in
+           re.finditer(r"(\w+): pairs=\d+ records=(\d+) tier0=\d+ tier1=(\d+) tier2=(\d+) bad=\d+ edge_start=\d+ edge_end=\d+ short_seq=\d+ lookup_at_start=\d+ "
+                       r"unstaged=(\d+) second_pass=(\d+) mm256=(\d+) max_smem=(\d+) cluster_launches=(\d+)", out.stdout)}
+    # per run, at least: (records, pairs in the second tier, pairs in the last tier, unstaged front-end tiles, reads clustered by
+    # cluster_kernel's second pass, reads of mapped pairs with 256 or more minimizers); then the number of cluster launches
+    floors = {"grown_chip192": (60, 20, 0, 0, 1, 0, 2), "grown_chip256": (75, 20, 0, 0, 1, 0, 2), "grown_chip448": (45, 15, 1, 0, 1, 0, 2),
+              "grown_chip704": (75, 30, 0, 1, 8, 0, 2), "grown_chip736": (50, 15, 0, 1, 0, 0, 1), "grown_chip832": (110, 80, 8, 1, 0, 2, 1),
+              "grown_atac256": (40, 20, 0, 0, 0, 0, 2), "grown_single_end320": (75, 15, 0, 0, 1, 0, 2), "grown_hic256": (45, 15, 0, 0, 0, 0, 2),
+              "grown_hic256_cta": (18, 18, 8, 0, 0, 0, 1), "grown_sam256": (50, 15, 0, 0, 0, 0, 2), "grown_sam_single_end320": (55, 15, 0, 0, 1, 0, 2),
+              "grown_k23_w11_320": (60, 20, 0, 0, 1, 0, 2), "grown_small_tiers256": (40, 35, 20, 0, 0, 0, 1)}
+    assert sorted(got) == sorted(floors), out.stdout
+    for name, (*floor, launches) in floors.items():
+        g = got[name]
+        assert all(x >= f for x, f in zip(g[:6], floor)) and g[7] == launches and g[6] <= 232448, (name, out.stdout)
+    # the front end's tiles at 832 bases: 4 x (64 x 832 + 32) + 16 x 128 x 8 bytes, the largest request of any launch there
+    assert got["grown_chip832"][6] == 229504, out.stdout
+    total = [sum(g[i] for g in got.values()) for i in (3, 4, 5)]
+    assert total[0] >= 4 and total[1] >= 25 and total[2] >= 2, (total, out.stdout)
