@@ -1614,6 +1614,9 @@ int orc_minimizers(const char *seq, uint32_t len, uint32_t seq_index, int k, int
 }
 int orc_banded_align(int e, const char *pattern, const char *text, int read_len, int *end_pos) { return banded_align(e, pattern, text, read_len, end_pos); }
 void orc_banded_traceback(int e, int min_errors, const char *pattern, const char *text, int read_len, int *start_pos) { banded_traceback(e, min_errors, pattern, text, read_len, start_pos); }
+int orc_adjust_gap_beginning(int strand, const char *ref, const char *read, int *gap, int read_end, int ref_start, int ref_end) {
+  return adjust_gap_beginning(strand, ref, read, gap, read_end, ref_start, ref_end);
+}
 // the mate-guided lookup (index.cc:351-489) over records that were probed elsewhere, for tests of the device formulations:
 // kind[i] 0 absent / 1 singleton / 2 multi, val[i] the table value, mm_hit[i] = read position << 1 | strand
 int orc_rescue_test(int k, int w, int max_seed_freq0, int min_num_seeds, int strand, uint32_t range, int n_mm, const uint8_t *kind,

@@ -84,6 +84,8 @@ int orc_banded_align(int e, const char *pattern, const char *text, int read_len,
 void orc_banded_traceback(int e, int min_errors, const char *pattern, const char *text, int read_len,
                           int *start_pos);
 int orc_align_dropoff(int e, const char *pattern, const char *text, int read_len, int from_3_end, int *end_pos, int *read_len_out);
+// alignment.cc:24-83: extend an exact match into the skipped 5' gap of a split alignment (raw, signed char compares).
+int orc_adjust_gap_beginning(int strand, const char *ref, const char *read, int *gap, int read_end, int ref_start, int ref_end);
 
 // One PE record as emitted by mapping_generator.cc:110-123 (before sort/dedup).
 typedef struct {

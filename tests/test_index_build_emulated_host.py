@@ -4,7 +4,8 @@ khash upload kernels `khash_count_kernel` / `khash_insert_kernel`) run UNCHANGED
 `build_index_on_device`'s sequence, std::sort / a prefix sum playing CUB, against the oracle's `orc_index_build`
 (Index::Construct, index.cc:12-89; shown equal to `chromap -i` by tests/test_oracle_golden.py): every key with its singleton
 flag and value, occurrence offsets and counts, the occurrence table entry by entry.  References with N runs, soft-masked
-bases, sequences shorter than a chunk and shorter than k, lengths off the chunk grid, tandem repeats, planted copies; three (k, w)."""
+bases, sequences shorter than a chunk and shorter than k, lengths off the chunk grid, tandem repeats, planted copies; three (k, w);
+and a reference holding every byte 0x01-0xFF but LF and CR (`base_code` against the oracle's CharToUint8 on all of them)."""
 from tests import emu
 
 MAIN = r'''
@@ -15,11 +16,25 @@ int main() {
   std::mt19937 g(101);
   long bad = 0, cases = 0, keys_total = 0, occ_total = 0;
   const int KW[3][2] = {{17, 7}, {21, 10}, {16, 5}};
-  for (int it = 0; it < 9; ++it) {
+  for (int it = 0; it < 10; ++it) {
     const int k = KW[it %% 3][0], w = KW[it %% 3][1];
     // ---- reference
     std::vector<std::string> seqs;
-    const int n_seq = 2 + (int)(g() %% 4);
+    if (it == 9) {   // every byte 0x01-0xFF but '\n' and '\r', 24 times each, between 30 random bases on either side
+      std::vector<int> mid;
+      for (int q = 0; q < 24; ++q) for (int b = 1; b < 256; ++b) if (b != 10 && b != 13) mid.push_back(b);
+      std::shuffle(mid.begin(), mid.end(), g);
+      for (size_t i = 0; i < mid.size(); i += 2000) {
+        std::string s;
+        for (size_t q = i; q < std::min(mid.size(), i + 2000); ++q) {
+          for (int x = 0; x < 30; ++x) s.push_back("ACGT"[g() %% 4]);
+          s.push_back((char)mid[q]);
+          for (int x = 0; x < 30; ++x) s.push_back("ACGT"[g() %% 4]);
+        }
+        seqs.push_back(s);
+      }
+    }
+    const int n_seq = it == 9 ? 0 : 2 + (int)(g() %% 4);
     for (int q = 0; q < n_seq; ++q) {
       size_t L = q == 0 ? 30000 + g() %% 9000 : q == 1 ? 2048 * 3 : q == 2 ? 10 + g() %% 30 : 300 + g() %% 5000;   // off the chunk grid, on it, shorter than k + w, shorter than a chunk
       std::string s(L, 'A');
@@ -27,12 +42,14 @@ int main() {
       seqs.push_back(s);
     }
     std::string &big = seqs[0];
-    std::string seg(700, 'A'); for (auto &c : seg) c = "ACGT"[g() %% 4];
-    for (int q = 0; q < 14; ++q) big.replace(100 + g() %% (big.size() - 1000), 700, seg);                       // planted copies: multi-occurrence keys
-    for (int i = 0; i < 600; ++i) big[5000 + i] = "ACG"[i %% 3];                                                // tandem repeat: ties inside a window
-    big.replace(9000, 120, std::string(120, 'N'));
-    big.replace(2040, 20, std::string(20, 'N'));                                                                // an N run across a chunk boundary
-    for (int q = 0; q < 2000; ++q) { const size_t at = g() %% big.size(); big[at] = (char)tolower(big[at]); }
+    if (it != 9) {   // planted copies, a tandem repeat, N runs and soft-masking in the first sequence
+      std::string seg(700, 'A'); for (auto &c : seg) c = "ACGT"[g() %% 4];
+      for (int q = 0; q < 14; ++q) big.replace(100 + g() %% (big.size() - 1000), 700, seg);                       // planted copies: multi-occurrence keys
+      for (int i = 0; i < 600; ++i) big[5000 + i] = "ACG"[i %% 3];                                                // tandem repeat: ties inside a window
+      big.replace(9000, 120, std::string(120, 'N'));
+      big.replace(2040, 20, std::string(20, 'N'));                                                                // an N run across a chunk boundary
+      for (int q = 0; q < 2000; ++q) { const size_t at = g() %% big.size(); big[at] = (char)tolower(big[at]); }
+    }
     std::string concat; std::vector<uint64_t> offs{0};
     for (auto &s : seqs) { concat += s; offs.push_back(concat.size()); }
     orc_reference *oref = orc_reference_from_memory((uint32_t)seqs.size(), concat.data(), offs.data(), nullptr);
@@ -114,4 +131,4 @@ def test_index_build_kernels_equal_the_oracles_index(tmp_path):
     out = emu.run(tmp_path, ["device_common.cuh", "index_build.cuh"], MAIN % dict(orc_h=emu.ORACLE_H), timeout=1200)
     assert out.returncode == 0 and "bad=0" in out.stdout, out.stdout[-2500:] + out.stderr[-800:]
     f = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
-    assert int(f["keys"]) > 50000 and int(f["occurrences"]) > 5000, out.stdout
+    assert int(f["references"]) == 10 and int(f["keys"]) > 50000 and int(f["occurrences"]) > 5000, out.stdout

@@ -48,7 +48,10 @@ int main(int argc, char **argv) {
       text += "read" + std::to_string(r);
       if (g() %% 2) text += (g() %% 2 ? " 1:N:0:ACGT" : "\tcomment");
       eol();
-      for (int i = 0; i < L; ++i) text.push_back("ACGTNacgt"[g() %% 9]);
+      for (int i = 0; i < L; ++i) {   // bases, and one byte in eight beyond them: 0x80-0xFF, '.', IUPAC codes in both cases
+        const u32 k = g() %% 8;
+        text.push_back(k ? "ACGTNacgt"[g() %% 9] : g() %% 2 ? (char)(0x80 + g() %% 128) : ".RYKMSWBDHVnrykmswbdhv"[g() %% 22]);
+      }
       eol();
       text += (defect == 2 && r == hit) ? "-" : (g() %% 2 ? "+" : "+read" + std::to_string(r));
       eol();

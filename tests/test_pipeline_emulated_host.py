@@ -95,13 +95,15 @@ struct RunStats {
   // g1 - base > tb); reads that cluster_kernel's first pass listed for the second; reads of mapped pairs with 256 or more
   // minimizers (the oracle's count: candidate counts are u8 and wrap there); the launches' largest dynamic shared memory
   long unstaged = 0, second_pass = 0, mm256 = 0, max_smem = 0, cluster_launches = 0;
+  // runs with `bytes`: oracle records whose read 1 has a lower-case base, by that read's strand field (0 / 1)
+  long lower_s0 = 0, lower_s1 = 0;
 };
 
 enum { MODE_CHIP = 0, MODE_ATAC = 1, MODE_HIC = 2, MODE_SE = 3, MODE_SAM = 4, MODE_SAM_SE = 5 };
 // mapping knobs over the preset (-1: the preset's value): -e, -s, -f f0,f1, --drop-repetitive-reads, --min-read-length
 struct Knobs { int e = -1, min_seeds = -1, f0 = -1, f1 = -1, drop_rep = -1, min_read_len = -1; };
 static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *caps3, int max_best, int read_len_base, bool front_only = false, int K = 17, int W = 7, int fam_copies = 90,
-                         const Knobs &kn = Knobs{}, bool edges = false, bool exact_len = false, int over_lo = 0, int over_hi = 0) {
+                         const Knobs &kn = Knobs{}, bool edges = false, bool exact_len = false, int over_lo = 0, int over_hi = 0, bool bytes = false) {
   // exact_len: every read read_len_base bases (no spread); over-long reads (one pair in twenty) of over_lo .. over_hi bases
   // (0: mrl + 5 .. mrl + 44)
   if (over_lo == 0) { over_lo = mrl + 5; over_hi = mrl + 44; }
@@ -116,6 +118,17 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   for (int q = 0; q < 12; ++q) { std::string &s = seq[g() %% 2]; s.replace(1000 + g() %% (s.size() - 4000), 2000, seg); }
   seq[0].replace(30000, 80, std::string(80, 'N'));
   for (int q = 0; q < 3000; ++q) { std::string &s = seq[g() %% 2]; const size_t at = g() %% s.size(); s[at] = (char)tolower(s[at]); }
+  if (bytes) {   // beyond upper-case ACGTN: soft-masked stretches of 50 to 2,000 bases over about 40 %%, IUPAC codes in both cases, bytes 0x80-0xFF
+    for (auto &s : seq) {
+      for (size_t masked = 0; masked < s.size() * 2 / 5;) {
+        const size_t ln = 50 + g() %% 1951, at = g() %% (s.size() - ln);
+        for (size_t i = at; i < at + ln; ++i) if (s[i] >= 'A' && s[i] <= 'Z') s[i] = (char)(s[i] + 32);
+        masked += ln;
+      }
+      for (size_t q = 0; q < s.size() / 400; ++q) s[g() %% s.size()] = "RYKMSWBDHVrykmswbdhv"[g() %% 20];
+      for (size_t q = 0; q < s.size() / 120; ++q) s[g() %% s.size()] = (char)(0x80 + g() %% 128);
+    }
+  }
   if (edges) {   // then many short sequences, as in a scaffold-level assembly: shorter than k + w - 1 (no minimizer), around L + 2e
                  // (no valid candidate), around a fragment, and a spread up to 3 kbp
     for (int len : {20, 30, 45, 60, 76, 80, 85, 90, 99, 100, 101, 110, 120, 136, 150, 180, 250, 400, 700, 1200, 3000}) seq.emplace_back((size_t)len, 'A');
@@ -176,7 +189,12 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
     }
     if (g() & 1) std::swap(a, b);
     for (std::string *r : {&a, &b}) {
-      for (auto &c : *r) c = (char)toupper(c);
+      const int deco = bytes ? (int)(g() %% 7) : -1;   // (bytes) one read in seven keeps the reference high bytes it was copied from, 32 lower
+      for (auto &c : *r) {
+        if (c >= 'a' && c <= 'z') c = (char)(c - 32);
+        // what a sequencer reads where the reference has no base; or (decoration 6) a high byte copied 32 lower, opposite its reference byte
+        if (bytes && !strchr("ACGTN", c)) c = deco == 6 && (u8)c >= 0x80 ? (char)((u8)c - 32) : "ACGT"[g() %% 4];
+      }
       const int ne = (int)(g() %% 4);
       for (int x = 0; x < ne; ++x) {
         const int k = (int)(g() %% 5), p2 = (int)(g() %% r->size());
@@ -187,6 +205,14 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
     }
     if ((int)a.size() != L1) a.resize((size_t)L1, 'A');
     if ((int)b.size() != L2) b.resize((size_t)L2, 'A');
+    for (std::string *r : {&a, &b}) {   // per read: none, wholly lower case, lower-case runs, 'n', '.', IUPAC codes (high bytes: above)
+      if (!bytes) break;
+      const int deco = (int)(g() %% 6), nr = (int)r->size();
+      auto lower = [](char &c) { if (c >= 'A' && c <= 'Z') c = (char)(c + 32); };
+      if (deco == 1) for (auto &c : *r) lower(c);
+      if (deco == 2) for (int q = 1 + (int)(g() %% 3); q > 0; --q) { const int ln = 5 + (int)(g() %% 36), at = (int)(g() %% (unsigned)std::max(1, nr - ln)); for (int i = at; i < std::min(nr, at + ln); ++i) lower((*r)[i]); }
+      if (deco >= 3) for (int q = 1 + (int)(g() %% 3); q > 0; --q) (*r)[g() %% nr] = deco == 3 ? 'n' : deco == 4 ? '.' : "RYKMSWBDHVrykmswbdhv"[g() %% 20];
+    }
     s1 += a; o1.push_back((u32)s1.size()); s2 += b; o2.push_back((u32)s2.size());
   }
   const int n = n_pairs;
@@ -210,6 +236,17 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
   std::vector<orc_pair_trace> trace((size_t)n);
   const long n_want = is_sam ? 0 : mode == MODE_SE ? (long)orc_map_reads_se(om, (u32)n, s1.data(), o1.data(), first_read_id, want.data(), (long)want.size(), 1)
                                       : (long)orc_map_pairs(om, (u32)n, s1.data(), o1.data(), s2.data(), o2.data(), first_read_id, want.data(), (long)want.size(), trace.data());
+  if (bytes) {
+    auto tally_lower = [&](u32 read_id, int strand) {
+      const u32 p = read_id - first_read_id;
+      bool lc = false;
+      for (u32 i = o1[p]; i < o1[p + 1]; ++i) lc |= s1[i] >= 'a' && s1[i] <= 'z';
+      if (lc) ++(strand ? rs.lower_s1 : rs.lower_s0);
+    };
+    if (is_sam) for (long i = 0; i < n_want_sam; ++i) tally_lower(want_sam[i].read_id, want_sam[i].strand[0]);
+    else if (mode == MODE_HIC) for (long i = 0; i < n_want; ++i) tally_lower(((const orc_pairs_record *)want.data())[i].read_id, ((const orc_pairs_record *)want.data())[i].strand1);
+    else for (long i = 0; i < n_want; ++i) tally_lower(want[i].read_id, want[i].direction);
+  }
   if (edges) {   // what the oracle mapped at the edges: [st, en) on rid, with the mate-guided lookup run or not
     const u32 L = (u32)read_len_base, e = (u32)op.error_threshold, range = (u32)op.max_insert_size;
     auto tally_edges = [&](u32 rid, u32 st, u32 en, bool looked_up) {
@@ -359,7 +396,16 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
              a.overflow == b.overflow;
         for (int m = 0; ok && m < (is_se ? 1 : 2); ++m) for (int q = 0; ok && q < a.n_cigar[m]; ++q) ok = a.cigar[m][q] == b.cigar[m][q];
       }
-      if (!ok) { if (rs.bad < 8) printf("SAM PAIR %%d (seed %%d): records %%d / %%d\n", p, seed, out_n[p], nw); ++rs.bad; }
+      if (!ok) {
+        if (rs.bad < 8) {
+          printf("SAM PAIR %%d (seed %%d): records %%d / %%d", p, seed, out_n[p], nw);
+          if (nw > 0 && out_n[p] > 0) { const OutSam &a = out_sam[(size_t)p * max_best]; const orc_sam_record &b = want_sam[w0];
+            for (int m = 0; m < (is_se ? 1 : 2); ++m) printf("  mate %%d pos %%u/%%u end %%u/%%u strand %%u/%%u n_cigar %%u/%%u", m, a.pos[m], b.pos[m], a.end[m], b.end[m], a.strand[m], b.strand[m], a.n_cigar[m], b.n_cigar[m]);
+            printf("  mapq %%u/%%u", a.mapq, b.mapq); }
+          printf("\n");
+        }
+        ++rs.bad;
+      }
     }
     if (si != n_want_sam) { printf("oracle SAM cores not consumed: %%ld of %%ld\n", si, n_want_sam); ++rs.bad; }
     orc_mapper_free(om); orc_index_free(oix); orc_reference_free(oref);
@@ -392,7 +438,7 @@ static RunStats run_case(int mode, int seed, int n_pairs, int mrl, const Caps *c
 int main(int argc, char **argv) {
   static_assert(sizeof(OutRecord) == sizeof(orc_pe_record) && sizeof(OutPairs) == sizeof(orc_pe_record), "record layouts");
   // the runs at the ends of reference sequences ("edges"), at the sizes a context grown beyond 160 bases takes ("grown"), else all others
-  const bool want_edges = argc > 1 && !strcmp(argv[1], "edges"), want_grown = argc > 1 && !strcmp(argv[1], "grown");
+  const bool want_edges = argc > 1 && !strcmp(argv[1], "edges"), want_grown = argc > 1 && !strcmp(argv[1], "grown"), want_bytes = argc > 1 && !strcmp(argv[1], "bytes");
   long bad = 0;
   const int mrl = 80;
   const Caps real[3] = {tier_caps(mrl, 0), tier_caps(mrl, 1), tier_caps(mrl, 2)};   // the library's tiers
@@ -401,7 +447,7 @@ int main(int argc, char **argv) {
   const Caps small_long[3] = {{150, 6, 2, 2}, {300, 40, 6, 6}, {600, 65536, 8192, 8192}};
   const Caps small_256[3] = {{256, 6, 2, 2}, {512, 40, 6, 6}, {1024, 65536, 8192, 8192}};
   struct Case { const char *name; int mode, seed, n, max_best, len; const Caps *caps; int mrl; bool front_only = false; int k = 17, w = 7, fam_copies = 90; Knobs knobs = {}; bool edges = false;
-                bool grown = false, exact = false; int over_lo = 0, over_hi = 0; };   // grown: caps nullptr = the library's tiers at mrl
+                bool grown = false, exact = false; int over_lo = 0, over_hi = 0; bool bytes = false; };   // grown: caps nullptr = the library's tiers at mrl
   const Case cases[] = {
       {"real_tiers", MODE_CHIP, 3, 100, 1, 60, real, mrl},
       {"small_first_tier", MODE_CHIP, 4, 48, 3, 60, small, mrl},
@@ -478,17 +524,30 @@ int main(int argc, char **argv) {
       // pairs through the CTA kernels at maxmm 512 / 1,024
       {.name = "grown_k23_w11_320", .mode = MODE_CHIP, .seed = 72, .n = 96, .max_best = 1, .len = 314, .caps = nullptr, .mrl = 320, .k = 23, .w = 11, .fam_copies = 30, .grown = true},
       {.name = "grown_small_tiers256", .mode = MODE_CHIP, .seed = 73, .n = 48, .max_best = 3, .len = 250, .caps = small_256, .mrl = 256, .fam_copies = 30, .grown = true},
+      // reads and a reference beyond upper-case ACGTN: the raw-byte compares (Hamming shortcut of the traceback, adapter trimming,
+      // Hi-C gap extension) and the case fold of every other step, in every mode, the CTA tiers and the 320-base SAM instance
+      {.name = "bytes_chip", .mode = MODE_CHIP, .seed = 80, .n = 160, .max_best = 1, .len = 100, .caps = nullptr, .mrl = 128, .bytes = true},
+      {.name = "bytes_chip_cta", .mode = MODE_CHIP, .seed = 81, .n = 64, .max_best = 2, .len = 60, .caps = small, .mrl = mrl, .bytes = true},
+      {.name = "bytes_atac", .mode = MODE_ATAC, .seed = 82, .n = 160, .max_best = 1, .len = 100, .caps = nullptr, .mrl = 128, .bytes = true},
+      {.name = "bytes_hic", .mode = MODE_HIC, .seed = 83, .n = 120, .max_best = 1, .len = 150, .caps = real_long, .mrl = 150, .bytes = true},
+      {.name = "bytes_hic_cta", .mode = MODE_HIC, .seed = 84, .n = 40, .max_best = 1, .len = 120, .caps = small_long, .mrl = 150, .bytes = true},
+      {.name = "bytes_single_end", .mode = MODE_SE, .seed = 85, .n = 160, .max_best = 2, .len = 100, .caps = nullptr, .mrl = 128, .bytes = true},
+      {.name = "bytes_sam", .mode = MODE_SAM, .seed = 86, .n = 120, .max_best = 2, .len = 100, .caps = nullptr, .mrl = 128, .over_lo = 133, .over_hi = 160,
+       .bytes = true},   // (SAM reads stay within the 160-base instance)
+      {.name = "bytes_sam_single_end", .mode = MODE_SAM_SE, .seed = 87, .n = 120, .max_best = 2, .len = 100, .caps = nullptr, .mrl = 128, .over_lo = 133, .over_hi = 160,
+       .bytes = true},   // (SAM reads stay within the 160-base instance)
+      {.name = "bytes_sam256", .mode = MODE_SAM, .seed = 88, .n = 64, .max_best = 2, .len = 250, .caps = nullptr, .mrl = 256, .fam_copies = 30, .bytes = true},
   };
   const int seed_off = getenv("EMU_SEED_OFFSET") ? atoi(getenv("EMU_SEED_OFFSET")) : 0;   // other inputs of the same kinds (offline fuzzing)
   for (const Case &c : cases) {
-    if (c.edges != want_edges || c.grown != want_grown) continue;
+    if (c.edges != want_edges || c.grown != want_grown || c.bytes != want_bytes) continue;
     Caps lib[3];
     for (int t = 0; t < 3; ++t) lib[t] = tier_caps(c.mrl, t);
     const RunStats r = run_case(c.mode, c.seed + seed_off, c.n, c.mrl, c.caps ? c.caps : lib, c.max_best, c.len, c.front_only, c.k, c.w, c.fam_copies, c.knobs, c.edges, c.exact,
-                                c.over_lo, c.over_hi);
+                                c.over_lo, c.over_hi, c.bytes);
     printf("%%s: pairs=%%ld records=%%ld tier0=%%ld tier1=%%ld tier2=%%ld bad=%%ld edge_start=%%ld edge_end=%%ld short_seq=%%ld lookup_at_start=%%ld unstaged=%%ld second_pass=%%ld "
-           "mm256=%%ld max_smem=%%ld cluster_launches=%%ld\n", c.name, r.pairs, r.records, r.tier_pairs[0], r.tier_pairs[1], r.tier_pairs[2], r.bad, r.edge_start, r.edge_end,
-           r.short_seq, r.lookup_at_start, r.unstaged, r.second_pass, r.mm256, r.max_smem, r.cluster_launches);
+           "mm256=%%ld max_smem=%%ld cluster_launches=%%ld lower_s0=%%ld lower_s1=%%ld\n", c.name, r.pairs, r.records, r.tier_pairs[0], r.tier_pairs[1], r.tier_pairs[2], r.bad, r.edge_start, r.edge_end,
+           r.short_seq, r.lookup_at_start, r.unstaged, r.second_pass, r.mm256, r.max_smem, r.cluster_launches, r.lower_s0, r.lower_s1);
     bad += r.bad;
     if (r.max_smem > 232448) { printf("%%s: a launch asks for %%ld B of dynamic shared memory, more than an H100 grants a CTA (232,448 B)\n", c.name, r.max_smem); ++bad; }
   }
@@ -584,3 +643,22 @@ def test_device_pipeline_at_grown_read_lengths_equals_the_oracle(tmp_path):
     assert got["grown_chip832"][6] == 229504, out.stdout
     total = [sum(g[i] for g in got.values()) for i in (3, 4, 5)]
     assert total[0] >= 4 and total[1] >= 25 and total[2] >= 2, (total, out.stdout)
+
+
+def test_device_pipeline_on_raw_bytes_equals_the_oracle(tmp_path):
+    """A soft-masked reference (about 40 %) with IUPAC codes in both cases and bytes 0x80-0xFF; reads that are wholly or partly
+    lower case, carry 'n', '.' or IUPAC codes, or a reference high byte copied 32 lower: the raw-byte compares of the Hamming
+    shortcut in the traceback, adapter trimming and the Hi-C gap extension, and the case fold (base_code) everywhere else.
+    Chip with the library's tiers and tiny ones, atac, Hi-C in the thread and the CTA form, single-end, `--SAM` paired and
+    single-end, and 2x250 `--SAM` through the 320-base instance; each against the oracle pair by pair."""
+    out = _run_cases(tmp_path, ["bytes"])
+    got = {m.group(1): [int(x) for x in m.groups()[1:]] for m in
+           re.finditer(r"(\w+): pairs=\d+ records=(\d+) tier0=\d+ tier1=(\d+) tier2=(\d+) .* lower_s0=(\d+) lower_s1=(\d+)", out.stdout)}
+    # per run, at least: (records, pairs in the second tier, pairs in the last tier, records whose read 1 has a lower-case base with
+    # strand field 0, the same with 1): about half of what the first run showed
+    floors = {"bytes_chip": (59, 34, 0, 14, 22), "bytes_chip_cta": (25, 17, 13, 7, 7), "bytes_atac": (43, 35, 0, 16, 12), "bytes_hic": (53, 49, 0, 3, 31),
+              "bytes_hic_cta": (17, 18, 12, 1, 10), "bytes_single_end": (82, 27, 0, 19, 35), "bytes_sam": (56, 29, 0, 13, 23),
+              "bytes_sam_single_end": (60, 19, 0, 12, 22), "bytes_sam256": (17, 12, 0, 5, 6)}
+    assert sorted(got) == sorted(floors), out.stdout
+    for name, floor in floors.items():
+        assert all(g >= f for g, f in zip(got[name], floor)), (name, out.stdout)

@@ -240,3 +240,27 @@ def test_soft_masked_reference_inside_md(emu_exe, tmp_path):
         masked.append(s)
     want = _check(emu_exe, tmp_path, p, names, masked, cores, None, 0, r1, r2)
     assert len(re.findall(rb"MD:Z:[0-9ACGT^]*[acgt]", want)) > 100
+
+
+BYTES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "synth_bytes")
+
+
+@pytest.mark.parametrize("case,reads,paired", [("pe_q0.sam", "pe100", True), ("se_q0.sam", "pe100", False), ("pe250_q0.sam", "pe250", True)])
+def test_cores_on_raw_bytes(emu_exe, tmp_path, case, reads, paired):
+    """Reads with lower case, 'n', '.', IUPAC codes and high bytes on a soft-masked reference with IUPAC codes and bytes 0x80-0xFF
+    (tests/golden/synth_bytes): the minus-strand SEQ turns every byte that is no base into 'N', NM / MD compare the read's raw
+    bytes against the reference folded to upper case and print the reference bytes as stored.  Device text == host twin ==
+    the reference binary's output."""
+    names, seqs = read_fasta(os.path.join(BYTES, "ref.fa.gz"))
+    ref = orc.Reference(os.path.join(BYTES, "ref.fa.gz"))
+    s1, o1, s2, o2 = load_pairs(BYTES, reads + "_1.fq.gz", reads + "_2.fq.gz")
+    cores = orc.map_sam_cores(orc.make_params("", mapq_threshold=0), orc.Index(ref=ref, k=17, w=7), ref, s1, o1,
+                              s2 if paired else None, o2 if paired else None).view(cb.SAM_RECORD)
+    split = lambda r: ([a for a, _, _ in r], [b for _, b, _ in r], [c for _, _, c in r])
+    r1 = split(read_fastq_records(os.path.join(BYTES, reads + "_1.fq.gz")))
+    r2 = split(read_fastq_records(os.path.join(BYTES, reads + "_2.fq.gz"))) if paired else None
+    p = cb.make_params("", max_read_length=256, output_format=4, single_end=int(not paired), mapq_threshold=0)
+    want = _check(emu_exe, tmp_path, p, names, seqs, cores, None, 0, r1, r2)
+    assert want == gzip.open(os.path.join(BYTES, case + ".gz")).read()
+    # the bytes reached the text: MD strings that name lower-case or high reference bytes
+    assert len(re.findall(rb"MD:Z:[^\t\n]*[acgt\x80-\xff]", want)) > 100
